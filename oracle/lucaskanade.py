@@ -64,7 +64,9 @@ def good_features_to_track(q, mask, max_corners=1000, quality_level=0.01, min_di
     """cv2.goodFeaturesToTrack(q, maxCorners, qualityLevel, minDistance, mask, blockSize=5)
     -> (P,2) float32 (x, y): threshold at quality*max over the mask, 3x3 local maxima off
     the 1-px border, sort by value descending (ties: larger raster address first), greedy
-    acceptance with squared distance >= minDistance^2 to every accepted corner."""
+    acceptance with squared distance >= minDistance^2 to every accepted corner.  Like cv2 the
+    threshold minDistance^2 is formed in double and compared with the float sum
+    dx*dx + dy*dy; that sum is the exact integer up to 2^24 and rounds above it."""
     if eig is None:
         eig = corner_min_eigen_val(q)
     H, W = eig.shape
@@ -94,14 +96,17 @@ def good_features_to_track(q, mask, max_corners=1000, quality_level=0.01, min_di
         cell = int(round(min_distance))
         gw, gh = (W + cell - 1) // cell, (H + cell - 1) // cell
         grid = {}
-        md2 = min_distance * min_distance
+        md2 = float(min_distance) * float(min_distance)
         for y, x in zip(ys.tolist(), xs.tolist()):
             xc, yc = x // cell, y // cell
             good = True
             for yy in range(max(0, yc - 1), min(gh - 1, yc + 1) + 1):
                 for xx in range(max(0, xc - 1), min(gw - 1, xc + 1) + 1):
                     for (px, py) in grid.get((yy, xx), ()):
-                        if (x - px) ** 2 + (y - py) ** 2 < md2:
+                        d2 = (x - px) ** 2 + (y - py) ** 2
+                        if d2 > 1 << 24:  # float squares, float sum
+                            d2 = float(np.float32((x - px) ** 2) + np.float32((y - py) ** 2))
+                        if d2 < md2:
                             good = False
                             break
                     if not good:

@@ -7,9 +7,9 @@
 // and off the 1-pixel border, (4) sorts them by value descending (ties: larger raster
 // address first), (5) accepts greedily if the squared distance to every accepted corner is
 // >= minDistance^2, stopping at maxCorners.  Steps 1-3 are streaming passes; 4 is a bitonic
-// sort of 64-bit keys (value bits << 32 | address); 5 is inherently ordered and runs as one
-// warp that tests 32 candidates at a time against a cell grid and resolves the order inside
-// the batch with shuffles -- results are identical to the sequential loop.
+// sort of 64-bit keys (order-preserving value bits << 32 | address); 5 is inherently ordered
+// and runs as one warp that tests 32 candidates at a time against a cell grid and resolves the
+// order inside the batch with shuffles -- results are identical to the sequential loop.
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -62,6 +62,15 @@ masked_max_final(const float *__restrict__ part, int nparts, double quality, uns
 }
 
 // ---- (2)+(3) threshold, 3x3 local maximum, mask, border; compact to keys ----------------
+// Unsigned key in the order of the float value: every bit of a negative value flipped, only the
+// sign bit of a positive one.  Candidates are negative when the masked maximum is (cornerMinEigenVal
+// returns values like -1.5e-8 on straight edges) and quality > 1 puts the threshold below it.
+// Never 0, the padding key, for a candidate (that would need the NaN 0xffffffff).
+__device__ __forceinline__ unsigned order_key(float v) {
+    const unsigned u = __float_as_uint(v);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
 __global__ void __launch_bounds__(TX *TY)
 candidates_kernel(const float *__restrict__ eig, const uint8_t *__restrict__ valid, int h, int w,
                   unsigned *__restrict__ state, unsigned long long *__restrict__ keys, unsigned cap) {
@@ -83,7 +92,7 @@ candidates_kernel(const float *__restrict__ eig, const uint8_t *__restrict__ val
         }
     if (!ismax) return;
     const unsigned slot = atomicAdd(&state[1], 1u);
-    if (slot < cap) keys[slot] = ((unsigned long long)__float_as_uint(v) << 32) | (unsigned)i;
+    if (slot < cap) keys[slot] = ((unsigned long long)order_key(v) << 32) | (unsigned)i;
 }
 
 // ---- (4) bitonic sort, descending, of n = 2^p keys (padding keys are 0) ----------------
@@ -133,12 +142,21 @@ bitonic_global_kernel(unsigned long long *__restrict__ keys, unsigned n, unsigne
 // ---- (5) ordered greedy min-distance selection ---------------------------------------------
 constexpr int CELL_CAP = 8;
 
+// cv::goodFeaturesToTrack's distance test: squares and sum in float, compared in double with
+// minDistance^2 squared in double.  A float threshold differs whenever minDistance^2 is not a float
+// (minDistance = sqrt(50): 50 passes a float threshold, fails cv2's).  The intrinsics keep any
+// build from fusing a multiply-add, which would round the sum differently above 2^24.
+__device__ __forceinline__ bool too_close(float dx, float dy, double md2) {
+    return (double)__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) < md2;
+}
+
 struct SelectParams {
     const unsigned long long *keys;
     const unsigned *state;  // [1] = number of candidates
     unsigned cap;
     int h, w, max_corners;
-    float min_distance;
+    double md2;             // minDistance^2, in double
+    bool use_dist;          // minDistance >= 1: otherwise every candidate is accepted
     int cell, gw, gh;
     int *cell_cnt;      // (gh*gw), zeroed
     short2 *cell_pts;   // (gh*gw*CELL_CAP)
@@ -149,7 +167,6 @@ struct SelectParams {
 __global__ void __launch_bounds__(32) select_kernel(const SelectParams p) {
     const int lane = threadIdx.x;
     const unsigned ncand = min(p.state[1], p.cap);
-    const float md2 = p.min_distance * p.min_distance;
     int accepted = 0;
     const bool limited = p.max_corners > 0;
     for (unsigned basei = 0; basei < ncand; basei += 32) {
@@ -162,7 +179,7 @@ __global__ void __launch_bounds__(32) select_kernel(const SelectParams p) {
             x = addr - y * p.w;
         }
         const int xc = x / p.cell, yc = y / p.cell;
-        if (ok && p.min_distance >= 1.f) {
+        if (ok && p.use_dist) {
             const int x1 = max(0, xc - 1), y1 = max(0, yc - 1);
             const int x2 = min(p.gw - 1, xc + 1), y2 = min(p.gh - 1, yc + 1);
             for (int yy = y1; yy <= y2 && ok; yy++)
@@ -171,8 +188,7 @@ __global__ void __launch_bounds__(32) select_kernel(const SelectParams p) {
                     const int cnt = min(p.cell_cnt[c], CELL_CAP);
                     for (int q = 0; q < cnt; q++) {
                         const short2 pt = p.cell_pts[c * CELL_CAP + q];
-                        const float dx = (float)(x - pt.x), dy = (float)(y - pt.y);
-                        if (dx * dx + dy * dy < md2) { ok = false; break; }
+                        if (too_close((float)(x - pt.x), (float)(y - pt.y), p.md2)) { ok = false; break; }
                     }
                 }
         }
@@ -180,10 +196,8 @@ __global__ void __launch_bounds__(32) select_kernel(const SelectParams p) {
         for (int i = 0; i < 32; i++) {
             const bool oki = __shfl_sync(0xffffffffu, ok, i);
             const int xi = __shfl_sync(0xffffffffu, x, i), yi = __shfl_sync(0xffffffffu, y, i);
-            if (oki && lane > i && ok && p.min_distance >= 1.f) {
-                const float dx = (float)(x - xi), dy = (float)(y - yi);
-                if (dx * dx + dy * dy < md2) ok = false;
-            }
+            if (oki && lane > i && ok && p.use_dist && too_close((float)(x - xi), (float)(y - yi), p.md2))
+                ok = false;
         }
         const unsigned bal = __ballot_sync(0xffffffffu, ok);
         const int rank = __popc(bal & ((1u << lane) - 1u));
@@ -200,14 +214,14 @@ __global__ void __launch_bounds__(32) select_kernel(const SelectParams p) {
             const int o = accepted + rank;
             p.out_xy[2 * o] = (float)x;
             p.out_xy[2 * o + 1] = (float)y;
-            if (p.min_distance >= 1.f) {
+            if (p.use_dist) {
                 const int slot = p.cell_cnt[c] + before;
                 if (slot < CELL_CAP) p.cell_pts[c * CELL_CAP + slot] = make_short2((short)x, (short)y);
             }
         }
         __syncwarp();
         // publish the new per-cell counts after every lane has read the old ones
-        if (take && p.min_distance >= 1.f) atomicAdd(&p.cell_cnt[c], 1);
+        if (take && p.use_dist) atomicAdd(&p.cell_cnt[c], 1);
         __threadfence_block();
         __syncwarp();
         accepted += __popc(bal);
@@ -243,9 +257,9 @@ __global__ void __launch_bounds__(32 * SEL_WARPS) select_smem_kernel(const Selec
     __syncthreads();
     const unsigned ncand = min(p.state[1], p.cap);
     const unsigned nbatch = (ncand + 31u) / 32u;
-    const float md2 = p.min_distance * p.min_distance;
-    // integer form of d2 < md2 for the all-pairs test (d2 is an exact integer; images < 32768 px a side)
-    const unsigned md2i = (unsigned)ceilf(md2);
+    // integer form of d2 < md2 for the all-pairs test: d2 is an exact integer (images < 32768 px a side),
+    // and below 2^24 (minDistance < 32.5 here) cv2's float sum of squares is that integer
+    const unsigned md2i = (unsigned)ceil(p.md2);
     const bool limited = p.max_corners > 0;
     for (unsigned b = warp; b < nbatch; b += SEL_WARPS) {
         // ---- preparation: independent of every other batch
@@ -293,9 +307,8 @@ __global__ void __launch_bounds__(32 * SEL_WARPS) select_smem_kernel(const Selec
                 const int ox = (xc + k % 3 - 1) * p.cell, oy = (yc + k / 3 - 1) * p.cell;
                 for (int q = 0; q < cnt; q++) {
                     const unsigned f = (wd >> (2 + 10 * q)) & 0x3ffu;
-                    const float dx = (float)(x - (ox + (int)(f & 31u)));
-                    const float dy = (float)(y - (oy + (int)(f >> 5)));
-                    if (dx * dx + dy * dy < md2) ok = false;
+                    if (too_close((float)(x - (ox + (int)(f & 31u))), (float)(y - (oy + (int)(f >> 5))), p.md2))
+                        ok = false;
                 }
             }
         }
@@ -428,14 +441,15 @@ extern "C" int b200_good_features(const float *eig, const uint8_t *valid, int m,
     sp.cap = ncand;
     sp.h = m; sp.w = n;
     sp.max_corners = max_corners;
-    sp.min_distance = (float)min_distance;
-    sp.cell = min_distance >= 1.0 ? (int)lrint(min_distance) : 1;
+    sp.md2 = min_distance * min_distance;  // in double, like cv2
+    sp.use_dist = min_distance >= 1.0;
+    sp.cell = sp.use_dist ? (int)lrint(min_distance) : 1;
     sp.gw = (n + sp.cell - 1) / sp.cell;
     sp.gh = (m + sp.cell - 1) / sp.cell;
     const size_t ncell = (size_t)sp.gw * sp.gh;
     sp.out_xy = out_xy;
     sp.out_count = out_count;
-    if (min_distance >= 1.0 && sp.cell <= 32 && ncell * sizeof(unsigned) <= 200 * 1024) {
+    if (sp.use_dist && sp.cell <= 32 && ncell * sizeof(unsigned) <= 200 * 1024) {
         const size_t smem = (ncell + 2) * sizeof(unsigned);  // the grid + the token and the running count
         B200_CUDA(cudaFuncSetAttribute(select_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         select_smem_kernel<<<1, 32 * SEL_WARPS, smem, s>>>(sp);

@@ -69,7 +69,8 @@ def test_morph_and_zoom(vet, golden):
     assert np.abs(w - golden["morph/image"]).max() < 1e-12 and np.array_equal(wm, golden["morph/mask"])
     w2, wm2 = vet.morph(np.ma.masked_where(img > 20, img), golden["morph/disp"])
     o2, om2 = ora.warp(img, (img > 20).astype(np.int8), golden["morph/disp"])
-    assert_bits_equal(w2, o2, "masked morph") and np.array_equal(wm2, om2)
+    assert_bits_equal(w2, o2, "masked morph")
+    assert np.array_equal(wm2, om2), "masked morph mask"
     rng = np.random.default_rng(0)
     for (c, h, w_, oh, ow_) in [(2, 2, 2, 4, 4), (2, 16, 16, 32, 32), (2, 3, 5, 7, 64), (2, 32, 32, 2048, 2048),
                                 (2, 32, 16, 504, 1016)]:
