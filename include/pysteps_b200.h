@@ -325,6 +325,34 @@ int b200_idw_fill(const double *xy, const double *vals, const int *npts_dev, int
                   const double *xgrid, int nx, const double *ygrid, int ny,
                   int coords_on_16th_grid, double *out, void *stream);
 
+/* What dense_lucaskanade decides about its declustered vectors before the interpolation
+ * (lucaskanade.py:245-269, decorators.py:190-208), computed on the device so that the fill is
+ * enqueued without a read-back.  48 bytes: the host copies it to pinned memory. */
+typedef struct {
+    int n_pool, n_kept, n_dec;  /* counts[0..2] of the sparse stage */
+    int nonfinite;              /* bit 0: a value (uv) is not finite, bit 1: a coordinate (xy) */
+    int mode;                   /* B200_IDW_ZERO / _CONSTANT / _INTERPOLATE / _REFUSED (non-finite input) */
+    int on_grid;                /* the coords_on_16th_grid level b200_idw_fill would be promised: 0, 1, 2 */
+    int n_fill;                 /* n_dec when mode == B200_IDW_INTERPOLATE, else 0 */
+    int pad;
+    double c0, c1;              /* the constant field (ZERO: 0, 0) */
+} B200IdwPlan;
+enum { B200_IDW_ZERO = 0, B200_IDW_CONSTANT = 1, B200_IDW_INTERPOLATE = 2, B200_IDW_REFUSED = 3 };
+
+/* counts = the sparse stage's (pool, kept, declustered) counts, xy/uv = the (cap, 2) declustered
+ * vectors.  Zero when no vector was pooled or declustered; constant (uv[0, :]) for one vector,
+ * (uv[0, 0], uv[0, 0]) when every value is equal; refused when a value or coordinate is not
+ * finite.  grid_ok != 0: every grid coordinate is an integer below 2^14 (on_grid may then be set). */
+int b200_idw_plan(const int *counts, const double *xy, const double *uv, int cap, int grid_ok,
+                  B200IdwPlan *plan, void *stream);
+/* b200_idw_fill for two variables with the plan on the device: vector count and path (zero or
+ * constant fill, 32-bit keys, packed or unpacked 64-bit keys) are taken from `plan` by the
+ * kernels, nothing is read back.  Grids and scratch are sized from npts_cap.  Fills out (2, ny, nx)
+ * and, when twin is not null, twin (ny, nx, 2) with the same values.  A refused plan writes nothing. */
+int b200_idw_fill_planned(const double *xy, const double *vals, const B200IdwPlan *plan, int npts_cap,
+                          int k, double power, double dist_offset, const double *xgrid, int nx,
+                          const double *ygrid, int ny, double *out, double *twin, void *stream);
+
 /* idwinterp2d with the k nearest vectors of every grid point found, ordered and weighted exactly
  * as the reference does it (scipy.spatial.cKDTree's query order, numpy's pairwise sum of the
  * weights, values accumulated in neighbour order): equal to the reference at EVERY grid point to

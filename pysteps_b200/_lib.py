@@ -94,6 +94,9 @@ _SIGNATURES = {
                                c_void_p, c_void_p]),
     "b200_idw_fill": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double,
                               c_double, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "b200_idw_plan": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "b200_idw_fill_planned": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_double, c_double, c_void_p,
+                                      c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "b200_idw_fill_ckdtree": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double,
                                       c_double, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "b200_vet_cost": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,

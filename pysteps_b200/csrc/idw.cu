@@ -39,10 +39,34 @@ struct IDWParams {
     int nx, ny;
     double power, offset, mean_res;
     double *out;  // (nvar, ny, nx)
+    double2 *twin;   // (ny, nx) pairs of the two variables, written beside `out` (or null; nvar == 2 only)
+    const B200IdwPlan *plan;  // device plan of b200_idw_fill_planned (or null: the host chose the kernel)
     int *tie_list;   // grid points whose k-th and (k+1)-th neighbours are equidistant (or null)
     int *tie_count;
     uint8_t *tile_done;  // per pixel tile: filled by the 32-bit-key kernel (or null)
 };
+
+// With a device plan several fill kernels are enqueued and each decides from the plan whether the
+// field is its own -- the choice the host makes from known counts in b200_idw_fill:
+//   KEY32   idw32_kernel<20>:           k_eff == 20, half-pixel grid, <= IDW_CHUNK vectors
+//   PACKED  idw_kernel<20, true, true>: k_eff == 20, 1/16 grid, <= IDW_CHUNK vectors (tiles KEY32 left)
+//   EXACT   idw_strided_kernel<20, true, false>: k_eff == 20 otherwise
+//   INSERT  idw_strided_kernel<32, false, ...>: k_eff != 20 (the K = 8 network of the host path gives the
+//           same bits: same list, same NumPy-order epilogue)
+// k_eff = min(k, npts).  npts is the plan's n_fill: 0 when the field is constant, zero or refused.
+enum { ROLE_KEY32, ROLE_PACKED, ROLE_EXACT, ROLE_INSERT };
+
+__device__ __forceinline__ bool plan_takes(const B200IdwPlan &pl, int k, int role) {
+    const int n = pl.n_fill;
+    if (n < 1) return false;
+    const bool k20 = min(k, n) == 20, pk = pl.on_grid >= 1 && n <= IDW_CHUNK;
+    switch (role) {
+        case ROLE_KEY32: return k20 && pk && pl.on_grid == 2;
+        case ROLE_PACKED: return k20 && pk;
+        case ROLE_EXACT: return k20 && !pk;
+        default: return !k20;
+    }
+}
 
 // numpy's pairwise summation for n < 128 (8 accumulators, then the remainder)
 template <int K>
@@ -192,12 +216,12 @@ struct TileBound {
 
 __device__ __forceinline__ TileBound tile_bound(const IDWParams &p, const double2 *__restrict__ pts, int npts, int k,
                                                 int *hist, int *fill, unsigned char *sbin, int *s_bmax,
-                                                int *s_total) {
+                                                int *s_total, int bx, int by) {
     const int tid = threadIdx.x, lane = tid & 31;
     TileBound tb;
     // ---- tile centre, half diagonal, histogram of centre distances ---------------------
-    const int j0 = blockIdx.x * IDW_TX, j1 = min(j0 + IDW_TX, p.nx) - 1;
-    const int i0 = blockIdx.y * IDW_TY, i1 = min(i0 + IDW_TY, p.ny) - 1;
+    const int j0 = bx * IDW_TX, j1 = min(j0 + IDW_TX, p.nx) - 1;
+    const int i0 = by * IDW_TY, i1 = min(i0 + IDW_TY, p.ny) - 1;
     const double xa = p.gx[j0], xb = p.gx[j1], ya = p.gy[i0], yb = p.gy[i1];
     tb.cx = 0.5 * (xa + xb);
     tb.cy = 0.5 * (ya + yb);
@@ -265,26 +289,27 @@ __device__ __forceinline__ TileBound tile_bound(const IDWParams &p, const double
 
 // FASTW: the weighting of dense_lucaskanade's call (two variables, power 1/2, unit resolution,
 // positive offset) from rsqrt; otherwise the general NumPy-order epilogue.
+// One pixel tile (bx, by) of idw_kernel.
 template <int K, bool EXACT, bool PACKED, bool FASTW>
-__global__ void __launch_bounds__(IDW_THREADS, FASTW ? 3 : 1) idw_kernel(const IDWParams p) {
+__device__ __forceinline__ void idw_tile(const IDWParams &p, int bx, int by, int tiles_x) {
     __shared__ double2 spt[IDW_CHUNK];
     __shared__ int sidx[IDW_CHUNK];
     __shared__ int hist[IDW_BINS];   // counts, then exclusive offsets
     __shared__ int fill[IDW_BINS];
     __shared__ unsigned char sbin[IDW_CHUNK];  // bin of the first IDW_CHUNK vectors
     __shared__ int s_bmax, s_total;
-    if (p.tile_done && p.tile_done[blockIdx.y * gridDim.x + blockIdx.x]) return;
+    if (p.tile_done && p.tile_done[by * tiles_x + bx]) return;
     const int npts = p.npts_dev ? min(*p.npts_dev, p.npts_cap) : p.npts_cap;
     const int k = min(min(p.k, npts), K);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     // a warp covers a compact 8x4 pixel patch: its lanes agree on most insert decisions
-    const int j = blockIdx.x * IDW_TX + (wid & 1) * 8 + (lane & 7);   // column
-    const int i = blockIdx.y * IDW_TY + (wid >> 1) * 4 + (lane >> 3);  // row
+    const int j = bx * IDW_TX + (wid & 1) * 8 + (lane & 7);   // column
+    const int i = by * IDW_TY + (wid >> 1) * 4 + (lane >> 3);  // row
     const double2 *__restrict__ pts = reinterpret_cast<const double2 *>(p.xy);
     const bool active = j < p.nx && i < p.ny;
     const double qx = p.gx[min(j, p.nx - 1)], qy = p.gy[min(i, p.ny - 1)];
 
-    const TileBound tb = tile_bound(p, pts, npts, k, hist, fill, sbin, &s_bmax, &s_total);
+    const TileBound tb = tile_bound(p, pts, npts, k, hist, fill, sbin, &s_bmax, &s_total, bx, by);
     const int bmax = tb.bmax, total = tb.total;
     auto bin_of = [&](int t) -> int { return tb.bin_of(pts, t); };
 
@@ -360,9 +385,10 @@ __global__ void __launch_bounds__(IDW_THREADS, FASTW ? 3 : 1) idw_kernel(const I
                 ay = fma(w, v.y, ay);
             }
         }
-        const double inv = 1.0 / ws;
-        p.out[((size_t)0 * p.ny + i) * p.nx + j] = ax * inv;
-        p.out[((size_t)1 * p.ny + i) * p.nx + j] = ay * inv;
+        const double inv = 1.0 / ws, fx = ax * inv, fy = ay * inv;
+        p.out[((size_t)0 * p.ny + i) * p.nx + j] = fx;
+        p.out[((size_t)1 * p.ny + i) * p.nx + j] = fy;
+        if (p.twin) p.twin[(size_t)i * p.nx + j] = make_double2(fx, fy);
         return;
     }
     double w[K];
@@ -386,6 +412,38 @@ __global__ void __launch_bounds__(IDW_THREADS, FASTW ? 3 : 1) idw_kernel(const I
             }
         p.out[((size_t)v * p.ny + i) * p.nx + j] = acc;
     }
+    if (p.twin) {  // this thread's own two stores, read back (keeps the K-wide loop's registers free)
+        const size_t g = (size_t)i * p.nx + j, N = (size_t)p.ny * p.nx;
+        p.twin[g] = make_double2(p.out[g], p.out[N + g]);
+    }
+}
+
+// one tile per CTA
+template <int K, bool EXACT, bool PACKED, bool FASTW>
+__global__ void __launch_bounds__(IDW_THREADS, FASTW ? 3 : 1) idw_kernel(const IDWParams p) {
+    if (p.plan && !plan_takes(*p.plan, p.k, EXACT ? (PACKED ? ROLE_PACKED : ROLE_EXACT) : ROLE_INSERT)) return;
+    idw_tile<K, EXACT, PACKED, FASTW>(p, blockIdx.x, blockIdx.y, gridDim.x);
+}
+
+// every CTA walks the tiles in steps of the grid size: b200_idw_fill_planned launches the kernels a plan
+// rarely chooses on one wave of resident CTAs, so that declining costs one wave instead of one per tile
+template <int K, bool EXACT, bool PACKED, bool FASTW>
+__global__ void __launch_bounds__(IDW_THREADS, FASTW ? 3 : 1) idw_strided_kernel(const IDWParams p) {
+    if (p.plan && !plan_takes(*p.plan, p.k, EXACT ? (PACKED ? ROLE_PACKED : ROLE_EXACT) : ROLE_INSERT)) return;
+    const int tiles_x = (p.nx + IDW_TX - 1) / IDW_TX, ntiles = tiles_x * ((p.ny + IDW_TY - 1) / IDW_TY);
+    for (int t = blockIdx.y * gridDim.x + blockIdx.x; t < ntiles; t += gridDim.x * gridDim.y) {
+        idw_tile<K, EXACT, PACKED, FASTW>(p, t % tiles_x, t / tiles_x, tiles_x);
+        __syncthreads();  // the next tile reuses the shared memory
+    }
+}
+
+// a grid of one wave of resident CTAs (at most one per tile)
+template <typename F>
+dim3 resident_grid(F kernel, dim3 full) {
+    int per_sm = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, IDW_THREADS, 0) != cudaSuccess || per_sm < 1)
+        per_sm = 1;
+    return dim3((unsigned)std::min<size_t>((size_t)full.x * full.y, (size_t)per_sm * b200::num_sms()));
 }
 
 // ---- 32-bit integer keys ---------------------------------------------------------------------
@@ -406,7 +464,8 @@ __global__ void __launch_bounds__(IDW_THREADS, 4) idw32_kernel(const IDWParams p
     __shared__ int fill[IDW_BINS];
     __shared__ unsigned char sbin[IDW_CHUNK];
     __shared__ int s_bmax, s_total;
-    const int npts = p.npts_cap;
+    if (p.plan && !plan_takes(*p.plan, p.k, ROLE_KEY32)) return;
+    const int npts = p.npts_dev ? min(*p.npts_dev, p.npts_cap) : p.npts_cap;
     const int k = K;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int j = blockIdx.x * IDW_TX + (wid & 1) * 8 + (lane & 7);   // column
@@ -414,7 +473,7 @@ __global__ void __launch_bounds__(IDW_THREADS, 4) idw32_kernel(const IDWParams p
     const double2 *__restrict__ pts = reinterpret_cast<const double2 *>(p.xy);
     const bool active = j < p.nx && i < p.ny;
     const double qx = p.gx[min(j, p.nx - 1)], qy = p.gy[min(i, p.ny - 1)];
-    const TileBound tb = tile_bound(p, pts, npts, k, hist, fill, sbin, &s_bmax, &s_total);
+    const TileBound tb = tile_bound(p, pts, npts, k, hist, fill, sbin, &s_bmax, &s_total, blockIdx.x, blockIdx.y);
     const int bmax = tb.bmax, total = tb.total;
     // every candidate lies within (bmax + 1) bins of the centre, every pixel within rt of it
     const double reach = 2.0 * ((double)(bmax + 1) * tb.binw + tb.rt) * (1.0 + 1e-6);
@@ -484,9 +543,75 @@ __global__ void __launch_bounds__(IDW_THREADS, 4) idw32_kernel(const IDWParams p
         ax = fma(w, v.x, ax);
         ay = fma(w, v.y, ay);
     }
-    const double inv = 1.0 / ws;
-    p.out[((size_t)0 * p.ny + i) * p.nx + j] = ax * inv;
-    p.out[((size_t)1 * p.ny + i) * p.nx + j] = ay * inv;
+    const double inv = 1.0 / ws, fx = ax * inv, fy = ay * inv;
+    p.out[((size_t)0 * p.ny + i) * p.nx + j] = fx;
+    p.out[((size_t)1 * p.ny + i) * p.nx + j] = fy;
+    if (p.twin) p.twin[(size_t)i * p.nx + j] = make_double2(fx, fy);
+}
+
+// ---- device plan (b200_idw_plan) -----------------------------------------------------------------
+// One CTA over the declustered vectors: the reference's early-outs and checks in their order
+// (lucaskanade.py:245-269, decorators.py:190-208) and the key level the host path derives from the
+// coordinates (xy * 16 integral with |xy| < 2^14; xy * 2 integral).
+__global__ void __launch_bounds__(1024)
+idw_plan_kernel(const int *__restrict__ counts, const double *__restrict__ xy, const double *__restrict__ uv,
+                int cap, int grid_ok, B200IdwPlan *__restrict__ plan) {
+    const int n_pool = counts[0], n_kept = counts[1];
+    const int n = max(min(counts[2], cap), 0);
+    const double u0 = n > 0 ? uv[0] : 0.0;
+    bool bad_uv = false, bad_xy = false, differ = false, off16 = false, off2 = false;
+    for (int t = threadIdx.x; t < 2 * n; t += blockDim.x) {
+        const double u = uv[t], x = xy[t];
+        bad_uv |= !isfinite(u);
+        bad_xy |= !isfinite(x);
+        differ |= !(u == u0);
+        const double x16 = x * 16.0, x2 = x * 2.0;
+        off16 |= !(x16 == rint(x16) && fabs(x) < 16384.0);
+        off2 |= !(x2 == rint(x2));
+    }
+    bad_uv = __syncthreads_or(bad_uv);
+    bad_xy = __syncthreads_or(bad_xy);
+    differ = __syncthreads_or(differ);
+    off16 = __syncthreads_or(off16);
+    off2 = __syncthreads_or(off2);
+    if (threadIdx.x != 0) return;
+    B200IdwPlan r;
+    r.n_pool = n_pool; r.n_kept = n_kept; r.n_dec = n;
+    r.nonfinite = (bad_uv ? 1 : 0) | (bad_xy ? 2 : 0);
+    r.on_grid = (grid_ok && !off16) ? (off2 ? 1 : 2) : 0;
+    r.n_fill = 0;
+    r.pad = 0;
+    r.c0 = r.c1 = 0.0;
+    if (n_pool == 0 || n == 0) {
+        r.mode = B200_IDW_ZERO;
+    } else if (bad_uv || bad_xy) {
+        r.mode = B200_IDW_REFUSED;
+    } else if (n == 1) {  // decorators.py:200-204
+        r.mode = B200_IDW_CONSTANT;
+        r.c0 = uv[0]; r.c1 = uv[1];
+    } else if (!differ) {  // decorators.py:207-208, max == min: the first value everywhere
+        r.mode = B200_IDW_CONSTANT;
+        r.c0 = r.c1 = u0;
+    } else {
+        r.mode = B200_IDW_INTERPOLATE;
+        r.n_fill = n;
+    }
+    *plan = r;
+}
+
+// the zero and constant fields of a plan, planar and (optionally) interleaved
+__global__ void __launch_bounds__(256)
+idw_plan_const_kernel(const B200IdwPlan *__restrict__ plan, double *__restrict__ out, double2 *__restrict__ twin,
+                      size_t N) {
+    const int mode = plan->mode;
+    if (mode != B200_IDW_ZERO && mode != B200_IDW_CONSTANT) return;
+    const double c0 = plan->c0, c1 = plan->c1;
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < N; e += stride) {
+        out[e] = c0;
+        out[N + e] = c1;
+        if (twin) twin[e] = make_double2(c0, c1);
+    }
 }
 
 // ---- k = None: every vector weighs in (interpolate.py:82-88, scipy cdist) ------------------------
@@ -585,6 +710,8 @@ extern "C" int b200_idw_fill(const double *xy, const double *vals, const int *np
     p.power = power; p.offset = dist_offset; p.mean_res = mean_res; p.out = out;
     p.tie_list = tie_list; p.tie_count = tie_count;
     p.tile_done = nullptr;
+    p.twin = nullptr;
+    p.plan = nullptr;
     dim3 grid(b200::ceil_div(nx, IDW_TX), b200::ceil_div(ny, IDW_TY));
     dim3 block(IDW_THREADS);
     // the host knows npts only as a capacity when npts_dev is given; EXACT needs k == K <= npts
@@ -613,7 +740,89 @@ extern "C" int b200_idw_fill(const double *xy, const double *vals, const int *np
     B200_LAUNCH_CHECK();
     B200_CUDA(cudaStreamWaitEvent(s, ss->join, 0));
     return kdp::idw_fix(xy, vals, nvar, k, power, dist_offset, mean_res, xgrid, nx, ygrid, ny, ts.tb, tie_list,
-                        tie_count, out, s);
+                        tie_count, out, nullptr, s);
+}
+
+extern "C" int b200_idw_plan(const int *counts, const double *xy, const double *uv, int cap, int grid_ok,
+                             B200IdwPlan *plan, void *stream) {
+    B200_REQUIRE(counts && xy && uv && plan && cap >= 1, "bad arguments");
+    idw_plan_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(counts, xy, uv, cap, grid_ok, plan);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+// b200_idw_fill with the vector count and the path taken from a device plan: every kernel that may
+// fill the field is enqueued (grids and scratch sized from the capacity) and all but the one the plan
+// chooses return at once (see plan_takes).  The path the plan chooses is the one b200_idw_fill takes
+// for the same vectors, so the field is the same bit for bit.
+extern "C" int b200_idw_fill_planned(const double *xy, const double *vals, const B200IdwPlan *plan, int npts_cap,
+                                     int k, double power, double dist_offset, const double *xgrid, int nx,
+                                     const double *ygrid, int ny, double *out, double *twin, void *stream) {
+    B200_REQUIRE(xy && vals && plan && xgrid && ygrid && out && npts_cap >= 1 && nx >= 1 && ny >= 1 && k >= 1,
+                 "bad arguments");
+    if (k > 32) {
+        b200::set_error("idw: k must be <= 32 (k=None / larger k is not implemented)");
+        return B200_ENOTSUP;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const size_t N = (size_t)ny * nx;
+    B200_REQUIRE(N < ((size_t)1 << 31), "grid too large");
+    {
+        const int blocks = (int)std::max<size_t>(1, std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 8));
+        idw_plan_const_kernel<<<blocks, 256, 0, s>>>(plan, out, (double2 *)twin, N);
+        B200_LAUNCH_CHECK();
+    }
+    kdp::TreeScratch ts;
+    b200::Scratch tie, done;
+    SideStream *ss = nullptr;
+    if (int rc = side_stream(&ss)) return rc;
+    if (int rc = kdp::tree_alloc(ts, npts_cap, s)) return rc;
+    B200_CUDA(tie.alloc(sizeof(int) * (N + 1), s));
+    int *tie_count = (int *)tie.p, *tie_list = tie_count + 1;
+    B200_CUDA(cudaMemsetAsync(tie_count, 0, sizeof(int), s));
+    B200_CUDA(cudaEventRecord(ss->fork, s));
+    B200_CUDA(cudaStreamWaitEvent(ss->s, ss->fork, 0));
+    // a tree of the n_fill vectors: empty unless the plan interpolates
+    if (int rc = kdp::tree_build(xy, &plan->n_fill, npts_cap, ts.tb, ss->s)) return rc;
+    B200_CUDA(cudaEventRecord(ss->join, ss->s));
+
+    IDWParams p;
+    memset(&p, 0, sizeof(p));
+    p.xy = xy; p.vals = vals; p.npts_dev = &plan->n_fill; p.npts_cap = npts_cap; p.nvar = 2; p.k = k;
+    p.gx = xgrid; p.gy = ygrid; p.nx = nx; p.ny = ny;
+    p.power = power; p.offset = dist_offset; p.mean_res = 1.0; p.out = out; p.twin = (double2 *)twin;
+    p.plan = plan;
+    p.tie_list = tie_list; p.tie_count = tie_count;
+    dim3 grid(b200::ceil_div(nx, IDW_TX), b200::ceil_div(ny, IDW_TY));
+    dim3 block(IDW_THREADS);
+    const bool fastw = power == 0.5 && dist_offset > 0.0;
+    if (k >= 20) {  // k_eff = min(k, n) can be 20: the register-resident K = 20 kernels
+        if (fastw) {
+            const size_t ntiles = (size_t)grid.x * grid.y;
+            B200_CUDA(done.alloc(ntiles, s));
+            B200_CUDA(cudaMemsetAsync(done.p, 0, ntiles, s));
+            p.tile_done = (uint8_t *)done.p;
+            idw32_kernel<20><<<grid, block, 0, s>>>(p);
+            B200_LAUNCH_CHECK();
+            idw_kernel<20, true, true, true><<<grid, block, 0, s>>>(p);
+            B200_LAUNCH_CHECK();
+            p.tile_done = nullptr;
+            auto *kx = idw_strided_kernel<20, true, false, true>;
+            kx<<<resident_grid(kx, grid), block, 0, s>>>(p);
+        } else {
+            idw_kernel<20, true, true, false><<<grid, block, 0, s>>>(p);
+            B200_LAUNCH_CHECK();
+            auto *kx = idw_strided_kernel<20, true, false, false>;
+            kx<<<resident_grid(kx, grid), block, 0, s>>>(p);
+        }
+        B200_LAUNCH_CHECK();
+    }
+    auto *ki = idw_strided_kernel<32, false, false, false>;
+    ki<<<resident_grid(ki, grid), block, 0, s>>>(p);
+    B200_LAUNCH_CHECK();
+    B200_CUDA(cudaStreamWaitEvent(s, ss->join, 0));
+    return kdp::idw_fix(xy, vals, 2, k, power, dist_offset, 1.0, xgrid, nx, ygrid, ny, ts.tb, tie_list,
+                        tie_count, out, (double2 *)twin, s);
 }
 
 extern "C" int b200_idw_fill_all(const double *xy, const double *vals, const int *npts_dev, int npts_cap, int nvar,

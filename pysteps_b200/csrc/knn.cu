@@ -444,6 +444,7 @@ struct IdwFixParams {
     kd::Item *nb;          // nthreads * k       (k > NBSMEM only)
     kd::NodeInfo *q;       // nthreads * QHEAP   (k > NBSMEM only)
     double *out;           // (nvar, ny, nx)
+    double2 *twin;         // (ny, nx) pairs of out's two variables, or null
 };
 
 // scipy's query and numpy's weighting (knn_body.cuh: idw_point) for the listed grid points, one
@@ -464,7 +465,10 @@ idw_fix_warp_kernel(const __grid_constant__ IdwFixParams p) {
         const size_t g = p.list_count ? (size_t)p.list[e] : e;
         const int i = (int)(g / p.nx), j = (int)(g % p.nx);
         warp_query(t, p.tb, p.xgrid[j], p.ygrid[i], k, ws, true, lane);
-        if (lane == 0) kd::idw_point(p.vals, p.nvar, ws.inds, ws.w, k, p.power, p.offset, p.mean_res, p.out + g, N);
+        if (lane == 0) {
+            kd::idw_point(p.vals, p.nvar, ws.inds, ws.w, k, p.power, p.offset, p.mean_res, p.out + g, N);
+            if (p.twin) p.twin[g] = make_double2(p.out[g], p.out[N + g]);
+        }
         __syncwarp();
     }
 }
@@ -489,6 +493,7 @@ idw_fix_kernel(const __grid_constant__ IdwFixParams p) {
         kdp::ArenaGrow grow(p.tb);
         kd::query(t, p.xgrid[j], p.ygrid[i], k, inds, nb, q, kdp::QHEAP, grow, w);
         kd::idw_point(p.vals, p.nvar, inds, w, k, p.power, p.offset, p.mean_res, p.out + g, N);
+        if (p.twin) p.twin[g] = make_double2(p.out[g], p.out[N + g]);
     }
 }
 
@@ -528,12 +533,12 @@ int tree_build(const double *xy, const int *n_dev, int n_cap, const TreeBuf &tb,
 
 int idw_fix(const double *xy, const double *vals, int nvar, int k, double power, double dist_offset,
             double mean_res, const double *xgrid, int nx, const double *ygrid, int ny, const TreeBuf &tb,
-            const int *list, const int *list_count, double *out, cudaStream_t s) {
+            const int *list, const int *list_count, double *out, double2 *twin, cudaStream_t s) {
     IdwFixParams p;
     memset(&p, 0, sizeof(p));
     p.xy = xy; p.vals = vals; p.xgrid = xgrid; p.ygrid = ygrid; p.nvar = nvar; p.k = k; p.nx = nx; p.ny = ny;
     p.power = power; p.offset = dist_offset; p.mean_res = mean_res; p.tb = tb;
-    p.list = list; p.list_count = list_count; p.out = out;
+    p.list = list; p.list_count = list_count; p.out = out; p.twin = nvar == 2 ? twin : nullptr;
     const size_t N = (size_t)ny * nx;
     if (k <= NBSMEM) {
         // as many warps as the chip holds (one search each); the list is usually shorter
@@ -582,7 +587,7 @@ extern "C" int b200_idw_fill_ckdtree(const double *xy, const double *vals, const
     if (int rc = kdp::tree_alloc(ts, npts_cap, s)) return rc;
     if (int rc = kdp::tree_build(xy, npts_dev, npts_cap, ts.tb, s)) return rc;
     return kdp::idw_fix(xy, vals, nvar, k, power, dist_offset, mean_res, xgrid, nx, ygrid, ny, ts.tb, nullptr,
-                        nullptr, out, s);
+                        nullptr, out, nullptr, s);
 }
 
 extern "C" int b200_detect_outliers(const double *uv, const double *xy, const int *n_dev, int n_cap,

@@ -68,9 +68,10 @@ struct ArenaGrow {
 
 int tree_alloc(TreeScratch &ts, int n_cap, cudaStream_t s);
 int tree_build(const double *xy, const int *n_dev, int n_cap, const TreeBuf &tb, cudaStream_t s);
-// recompute the listed grid points (list_count == nullptr: all of them) from scipy's query
+// recompute the listed grid points (list_count == nullptr: all of them) from scipy's query; twin (or
+// null, nvar == 2 only): the (ny, nx) pairs kept beside out, rewritten at the same points
 int idw_fix(const double *xy, const double *vals, int nvar, int k, double power, double dist_offset,
             double mean_res, const double *xgrid, int nx, const double *ygrid, int ny, const TreeBuf &tb,
-            const int *list, const int *list_count, double *out, cudaStream_t s);
+            const int *list, const int *list_count, double *out, double2 *twin, cudaStream_t s);
 
 }  // namespace kdp

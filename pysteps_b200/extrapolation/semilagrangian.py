@@ -101,6 +101,18 @@ def _known_finite(t):
     return v is not None and v == t._version
 
 
+def _valid_twin(t, m, n):
+    """The (m, n, 2) float64 copy dense_lucaskanade stores beside a device field it returns
+    (`_b200_twin`), while the field has not been written to since (`_b200_twin_version` still equals
+    its version counter), else None."""
+    tw = getattr(t, "_b200_twin", None)
+    if tw is None or getattr(t, "_b200_twin_version", None) != t._version:
+        return None
+    if t.dtype != torch.float64 or tuple(tw.shape) != (m, n, 2):
+        return None
+    return tw
+
+
 class _Stats:
     """[(n_nonfinite, nanmin, nanmax, n_nan), ...] of the given fields, reduced on the device.
     The kernels are enqueued at construction.  `post()` -- called once every kernel that writes a
@@ -312,7 +324,11 @@ def _extrapolate_checked(precip, velocity, d_precip, d_vel, stats, on_device, ti
     # trajectory kernel is timed alone.
     layout = _lib.LAYOUT_INTERLEAVED if interleaved else _lib.LAYOUT_PLANAR
     d_v = d_vel
-    if _lib._trace is not None and not interleaved:
+    twin = None if interleaved else _valid_twin(d_vel, m, n)
+    if twin is not None:
+        # the dense LK field's interleaved copy, written by the fill beside the planar field
+        d_v, layout = twin, _lib.LAYOUT_INTERLEAVED
+    elif _lib._trace is not None and not interleaved:
         d_v = torch.empty((m, n, 2), dtype=d_vel.dtype, device="cuda")
         _lib.call("b200_sl_interleave_velocity", d_vel.data_ptr(), _device.dtype_code(d_vel.dtype),
                   m, n, d_v.data_ptr(), _device.stream_ptr())

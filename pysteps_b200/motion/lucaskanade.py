@@ -159,6 +159,71 @@ def _pyramid_layout(m, n, win, max_level):
     return lv.value, int(tot.value)
 
 
+_KD_SHARED_MAX = 4096  # csrc/knn_device.cuh NMAX: the tree of the tie recomputation is built in one CTA
+_plan_pin = threading.local()
+
+
+def _fill_planned(interp_kwargs, counts, dec_xy, dec_uv, pool_cap, m, n, r0, r1, verbose):
+    """The interpolation stage of a device-resident dense call without a read-back in front of it:
+    b200_idw_plan derives the early-outs, checks and key level from the declustered vectors on the
+    device, b200_idw_fill_planned is enqueued behind it at once and its kernels follow the plan, and the
+    host reads the 48-byte plan while they run.  Raises and returns as the read-back path does;
+    returns (out, twin, whether the vectors reached the interpolator), or None for the shapes that path keeps: k=None, k outside 1..32, more pooled
+    vectors than the one-CTA tree build holds, fewer than two rows or columns, and interpolator
+    arguments that are not numbers (the read-back path raises on those only once it interpolates)."""
+    k = interp_kwargs.get("k", 20)
+    try:
+        power = float(interp_kwargs.get("power", 0.5))
+        dist_offset = float(interp_kwargs.get("dist_offset", 0.5))
+        k = None if k is None else int(k)
+    except (TypeError, ValueError):
+        return None
+    if k is None or not 1 <= k <= 32 or pool_cap > min(_DECLUSTER_MAX, _KD_SHARED_MAX) or m < 2 or n < 2:
+        return None
+    mb = r1 - r0
+    plan = torch.empty(12, dtype=torch.int32, device="cuda")  # B200IdwPlan, include/pysteps_b200.h
+    _call("b200_idw_plan", counts.data_ptr(), dec_xy.data_ptr(), dec_uv.data_ptr(), pool_cap,
+          int(max(m, n) < 16384), plan.data_ptr(), _s())
+    pin = getattr(_plan_pin, "buf", None)
+    if pin is None:
+        pin = _plan_pin.buf = torch.empty(12, dtype=torch.int32, pin_memory=True)
+    pin.copy_(plan, non_blocking=True)
+    ready = torch.cuda.Event()
+    ready.record()
+    out = torch.empty((2, mb, n), dtype=torch.float64, device="cuda")
+    twin = torch.empty((mb, n, 2), dtype=torch.float64, device="cuda")
+    xgrid, ygrid = _pixel_grid(0, n), _pixel_grid(r0, r1)
+    _call("b200_idw_fill_planned", dec_xy.data_ptr(), dec_uv.data_ptr(), plan.data_ptr(), pool_cap, k, power,
+          dist_offset, xgrid.data_ptr(), n, ygrid.data_ptr(), mb, out.data_ptr(), twin.data_ptr(), _s())
+    ready.synchronize()
+    n_pool, n_kept, n_dec, nonfinite = pin[:4].tolist()
+    # the read-back path's early-outs and errors, in its order (:245-269, decorators.py:190-208); a
+    # zero field is written by the fill itself
+    if n_pool == 0:
+        return out, twin, False
+    if verbose:
+        print("--- LK found %i sparse vectors ---" % n_kept)
+    if n_dec == 0:
+        return out, twin, False
+    if nonfinite & 1:
+        raise ValueError("argument 'values' contains non-finite values")
+    if nonfinite & 2:
+        raise ValueError("argument 'xy_coord' contains non-finite values")
+    return out, twin, True
+
+
+def _attach_twin(out, twin, interp_kwargs):
+    """The finiteness certificate (see the end of dense_lucaskanade) and the interleaved (m, n, 2) copy
+    of the field the extrapolator reads: both hold for THIS version of the returned tensor only (torch
+    bumps ._version on every in-place write, through views too)."""
+    power = float(interp_kwargs.get("power", 0.5))
+    dist_offset = float(interp_kwargs.get("dist_offset", 0.5))
+    if dist_offset > 0.0 and 0.0 <= power <= 8.0:
+        out._b200_finite_version = out._version
+    out._b200_twin = twin
+    out._b200_twin_version = out._version
+
+
 def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kwargs=None,
                       interp_method="idwinterp2d", interp_kwargs=None, dense=True,
                       nr_std_outlier=3, k_outlier=30, size_opening=3, decl_scale=20,
@@ -386,9 +451,21 @@ def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kw
               float(decl_scale), 1, dec_xy.data_ptr(), dec_uv.data_ptr(), counts[2:3].data_ptr(), _s())
     else:
         counts[2:3].copy_(counts[1:2])
+    if on_device and dense:
+        planned = _fill_planned(interp_kwargs, counts, dec_xy, dec_uv, pool_cap, m, n, r0, r1, verbose)
+        if planned is not None:
+            out, twin, filled = planned
+            if verbose and filled:
+                torch.cuda.current_stream().synchronize()
+                print("--- total time: %.2f seconds ---" % (time.time() - t0))
+            _attach_twin(out, twin, interp_kwargs)
+            return out
     # the one host read-back of the sparse stage: the counts AND (dense case) the declustered vectors the
     # interpolator's host-side checks look at, in one round trip -- three separate .cpu() calls were three
-    # waits with the GPU idle in between
+    # waits with the GPU idle in between.  A device-resident dense call takes the planned fill above
+    # instead; this path remains for sparse results (they are returned sized by the count), k=None (a
+    # different kernel), pools beyond the one-CTA tree build, and NumPy results, whose 64 MB (2048^2)
+    # download at the end waits for the whole fill anyway
     pin = _readback_buffers(pool_cap)
     pin[0].copy_(counts, non_blocking=True)
     if dense:
