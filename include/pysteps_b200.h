@@ -430,6 +430,37 @@ int b200_gaussian_filter(const double *in, int h, int w, const double *weights, 
 int b200_proesmans_field(const double *frames, int m, int n, double lam, int num_iter, int num_levels,
                          double *advfield, double *quality, void *stream);
 
+/* ------------------------------------------------------------------------
+ * Constant advection field (pysteps/motion/constant.py:41-49): the objective that
+ * scipy.optimize.minimize (Nelder-Mead, on the host) evaluates at every point it visits,
+ *   f(v) = -corrcoef(next[mask], warped[mask])[0, 1]
+ *   warped = map_coordinates(prev, [Y + vy, X + vx], order=0, mode="constant", cval=nan)
+ *   mask   = isfinite(next) & isfinite(warped)
+ * ---------------------------------------------------------------------- */
+
+/* bits of record[2]: the floating-point events of NumPy's corrcoef tail, in its order */
+#define B200_CONST_EMPTY 1         /* N == 0: "Mean of empty slice." and 0/0 in the mean */
+#define B200_CONST_DOF 2           /* N - 1 <= 0: "Degrees of freedom <= 0 for slice" and 1/0.0 */
+#define B200_CONST_SCALE_INVALID 4 /* c *= 1/fact: 0 * inf */
+#define B200_CONST_ROW_INVALID 8   /* c /= stddev[:, None]: invalid, divide by zero, overflow */
+#define B200_CONST_ROW_DIVZERO 16
+#define B200_CONST_ROW_OVERFLOW 32
+#define B200_CONST_COL_INVALID 64  /* c /= stddev[None, :] */
+#define B200_CONST_COL_DIVZERO 128
+#define B200_CONST_COL_OVERFLOW 256
+#define B200_CONST_SUM_BLOCKS 256  /* the centred sums: 256 CTAs x 256 threads, element i on lane i % 65536 */
+
+/* Bytes of device scratch b200_constant_eval needs for an (m, n) frame (written to *bytes, a host
+ * pointer).  The scratch must be zeroed before its first use; the evaluations leave it reusable. */
+int b200_constant_scratch_bytes(int m, int n, int64_t *bytes);
+/* One evaluation of f at (vx, vy) = (v[0], v[1]).  prev = R[-2], next = R[-1]: (m, n) device
+ * frames of `dtype` (float32 frames are widened, never narrowed).  Only enqueues kernels; record
+ * (device, 3 doubles) receives f, the number N of counted pixels and the B200_CONST_* bits.
+ * The means are NumPy's pairwise sums of the counted values in raster order, bit for bit; the
+ * centred sums are float64 in the fixed order of B200_CONST_SUM_BLOCKS. */
+int b200_constant_eval(const void *prev, const void *next, int dtype, int m, int n, double vx, double vy,
+                       void *scratch, double *record, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -109,6 +109,9 @@ _SIGNATURES = {
                               c_void_p]),
     "b200_zoom_bilinear": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200_field_stats": (c_int, [c_void_p, c_int, c_i64, c_void_p, c_void_p]),
+    "b200_constant_scratch_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_i64)]),
+    "b200_constant_eval": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_void_p,
+                                   c_void_p, c_void_p]),
     "b200_convert": (c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p]),
 }
 

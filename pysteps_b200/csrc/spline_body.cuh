@@ -164,6 +164,19 @@ SPL_FN long long tap_index(long long base, long long off, long long len, int mod
     return i < 0 ? 0 : (i >= len ? len - 1 : i);
 }
 
+// mode="constant": a coordinate outside [0, M-1] x [0, N-1] samples cval
+SPL_FN bool outside_grid(double cy, double cx, long long M, long long N) {
+    return !(cy >= 0.0 && cy <= (double)(M - 1) && cx >= 0.0 && cx <= (double)(N - 1));
+}
+
+// order 0: flat index of the nearest tap, floor(c + 0.5) on both axes (used by sample_pixel and by
+// the shifted-frame correlation of constant.cu)
+SPL_FN long long order0_index(double cy, double cx, long long M, long long N, int mode) {
+    const long long iy = tap_index(cast_floor(floor(add(cy, 0.5))), 0, M, mode);
+    const long long ix = tap_index(cast_floor(floor(add(cx, 0.5))), 0, N, mode);
+    return iy * N + ix;
+}
+
 // get_spline_interpolation_weights of scipy's ni_splines.c (orders 2..5): x becomes the offset from
 // the middle knot, the last weight is one minus the others
 SPL_FN void spline_weights(double x, int order, double *w) {
@@ -265,14 +278,11 @@ SPL_FN double sample_pixel(const SampleParams &p, int x, int yl, int t) {
     const double cy = add(cy0, (double)p.pad), cx = add(cx0, (double)p.pad);
     double v;
     bool outside = false;
-    if (p.mode == B200_MODE_CONSTANT)
-        outside = !(cy >= 0.0 && cy <= (double)(M - 1) && cx >= 0.0 && cx <= (double)(N - 1));
+    if (p.mode == B200_MODE_CONSTANT) outside = outside_grid(cy, cx, M, N);
     if (outside) {
         v = p.cval;
     } else if (p.order == 0) {
-        const long long iy = tap_index(cast_floor(floor(add(cy, 0.5))), 0, M, p.mode);
-        const long long ix = tap_index(cast_floor(floor(add(cx, 0.5))), 0, N, p.mode);
-        v = add(0.0, ld(p.coeffs + iy * N + ix));
+        v = add(0.0, ld(p.coeffs + order0_index(cy, cx, M, N, p.mode)));
     } else {
         const int order = p.order, half = p.order / 2;
         const long long by = cast_floor((order & 1) ? floor(cy) : floor(add(cy, 0.5)));

@@ -33,6 +33,8 @@ def methods():
         pass
     from .motion import proesmans
     out["motion"]["proesmans_b200"] = proesmans.proesmans
+    from .motion import constant
+    out["motion"]["constant_b200"] = constant.constant
     return out
 
 
@@ -41,8 +43,8 @@ def register(override=False):
 
     override=False: only the ``*_b200`` names are added (the identity checks of
     pysteps/tests/test_interfaces.py keep passing).  override=True additionally
-    replaces ``"semilagrangian"``, ``"lk"``/``"lucaskanade"``, ``"vet"`` and the noise
-    method ``"bps"``.
+    replaces ``"semilagrangian"``, ``"lk"``/``"lucaskanade"``, ``"vet"``, ``"proesmans"``,
+    ``"constant"`` and the noise method ``"bps"``.
     Returns the list of registered names.
     """
     import pysteps.extrapolation.interface as ei

@@ -3,7 +3,8 @@
 Same ``get_method(name)`` contract: case-insensitive names, ``None`` -> a callable that
 returns a zero field, unknown names -> ValueError, "brox"/"clg" -> NotImplementedError
 (pysteps/motion/interface.py:97-111).  "proesmans" is built but opt-in until verified on
-hardware (see motion/proesmans.py); darts, farneback and constant are not provided.
+hardware (see motion/proesmans.py); "constant" is motion/constant.py; darts and farneback are not
+provided.
 """
 import numpy as np
 
@@ -26,6 +27,11 @@ from .proesmans import proesmans  # noqa: E402
 
 _methods["proesmans"] = proesmans
 _methods["proesmans_b200"] = proesmans
+
+from .constant import constant  # noqa: E402
+
+_methods["constant"] = constant
+_methods["constant_b200"] = constant
 
 
 def get_method(name):
