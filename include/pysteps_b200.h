@@ -461,6 +461,39 @@ int b200_constant_scratch_bytes(int m, int n, int64_t *bytes);
 int b200_constant_eval(const void *prev, const void *next, int dtype, int m, int n, double vx, double vy,
                        void *scratch, double *record, void *stream);
 
+/* ------------------------------------------------------------------------
+ * DARTS (pysteps/motion/darts.py:22-220).  Complex arrays are interleaved float64 (re, im) pairs.
+ * The 50 x 50 solve (at the defaults) runs on the host; the device computes the block of the
+ * spectrum the reference reads, the normal equations MM = M^H M and M^H y, and the field.
+ * ---------------------------------------------------------------------- */
+#define B200_DARTS_MAX_COLS 242   /* n_c = 2 (2 M_x + 1)(2 M_y + 1): M_x, M_y <= 5 */
+#define B200_DARTS_MAX_SIDE 121   /* 2 M + 1 of one axis of the field's coefficients */
+#define B200_DARTS_NORMAL_ROWS 512 /* rows of M per partial of b200_darts_normal */
+
+/* The (Kt, Ky, 2K+1) complex block X[kt, ky, kx] = sum_{t,y,x} frames[t, y, x] tw_t[kt, t] tw_y[ky, y]
+ * tw_x(kx, x) of the (T, m, n) device frames of `dtype` (float32 is widened).  Host-built tables,
+ * exp(-2 pi i ((k j) mod L) / L) of the wrapped numpy index k: tw_t (Kt, T), tw_y (Ky, m) one row per
+ * block index, tw_x (fx, n) for the frequencies f = 0 .. fx-1 <= n / 2; block column kx = -K..K reads
+ * f = w or conj at f = n - w, w = kx mod n, whichever is <= n / 2.  Passes: x (real rows against tw_x,
+ * fixed order over x), t, y.  work: (T m fx + Kt m (2K+1)) complex.  The x pass reads the frames less
+ * frames[0, 0, 0]: only the DC coefficient changes, which M and y only ever multiply by zero
+ * (i_ = j_ = k_t = 0), and a constant stack gives an exactly zero block, as NumPy's FFT does. */
+int b200_darts_spectrum(const void *frames, int dtype, int T, int m, int n, const double *tw_x, int fx,
+                        const double *tw_y, int Ky, const double *tw_t, int Kt, int K, double *work,
+                        double *spectrum, void *stream);
+/* From the block of b200_darts_spectrum (Kt = 2 N_t + 1, Ky = 2 (N_y + M_y) + 1, Kx = 2 (N_x + M_x) + 1):
+ * mm (n_c, n_c) = M^H M and mhy (n_c) = M^H y, M's rows i = (k_t, k_y, k_x) in the reference's
+ * order, A scaled by sy * i_, B by sx * j_ (sy = c1 / T_y, sx = c1 / T_x), y = k_t X[k_y, k_x, k_t].
+ * work: ceil(rows / B200_DARTS_NORMAL_ROWS) * (n_c (n_c + 1) / 2 + n_c) complex partials,
+ * rows = (2 N_t + 1)(2 N_y + 1)(2 N_x + 1).  n_c <= B200_DARTS_MAX_COLS. */
+int b200_darts_normal(const double *spectrum, int N_x, int N_y, int N_t, int M_x, int M_y, double sx, double sy,
+                      double *work, double *mm, double *mhy, void *stream);
+/* out (2, m, n) float64 planar: out[c, y, x] = Re(sum_{a,b} coef[c, a, b] ey[a, y] ex[b, x]) / (m n),
+ * coef (2, h, w) complex, ey (h, m) and ex (w, n) the tables exp(+2 pi i ((k j) mod L) / L) of the
+ * coefficients' wrapped indices.  w <= B200_DARTS_MAX_SIDE. */
+int b200_darts_synthesize(const double *coef, int h, int w, const double *ey, const double *ex, int m, int n,
+                          double *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -112,7 +112,13 @@ _SIGNATURES = {
     "b200_constant_scratch_bytes": (c_int, [c_int, c_int, ctypes.POINTER(c_i64)]),
     "b200_constant_eval": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_void_p,
                                    c_void_p, c_void_p]),
-    "b200_convert": (c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p]),
+    "b200_darts_spectrum": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
+                                    c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b200_darts_normal": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_double, c_void_p,
+                                  c_void_p, c_void_p, c_void_p]),
+    "b200_darts_synthesize": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                      c_void_p]),
+    "b200_convert":(c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p]),
 }
 
 

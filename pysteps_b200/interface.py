@@ -35,6 +35,8 @@ def methods():
     out["motion"]["proesmans_b200"] = proesmans.proesmans
     from .motion import constant
     out["motion"]["constant_b200"] = constant.constant
+    from .motion import darts
+    out["motion"]["darts_b200"] = darts.DARTS
     return out
 
 
@@ -44,7 +46,7 @@ def register(override=False):
     override=False: only the ``*_b200`` names are added (the identity checks of
     pysteps/tests/test_interfaces.py keep passing).  override=True additionally
     replaces ``"semilagrangian"``, ``"lk"``/``"lucaskanade"``, ``"vet"``, ``"proesmans"``,
-    ``"constant"`` and the noise method ``"bps"``.
+    ``"constant"``, ``"darts"`` and the noise method ``"bps"``.
     Returns the list of registered names.
     """
     import pysteps.extrapolation.interface as ei

@@ -3,8 +3,8 @@
 Same ``get_method(name)`` contract: case-insensitive names, ``None`` -> a callable that
 returns a zero field, unknown names -> ValueError, "brox"/"clg" -> NotImplementedError
 (pysteps/motion/interface.py:97-111).  "proesmans" is built but opt-in until verified on
-hardware (see motion/proesmans.py); "constant" is motion/constant.py; darts and farneback are not
-provided.
+hardware (see motion/proesmans.py); "constant" is motion/constant.py; "darts" is motion/darts.py;
+farneback is not provided.
 """
 import numpy as np
 
@@ -32,6 +32,11 @@ from .constant import constant  # noqa: E402
 
 _methods["constant"] = constant
 _methods["constant_b200"] = constant
+
+from .darts import DARTS  # noqa: E402
+
+_methods["darts"] = DARTS
+_methods["darts_b200"] = DARTS
 
 
 def get_method(name):
