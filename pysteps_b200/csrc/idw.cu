@@ -18,6 +18,10 @@
 // equals it is appended to a list and recomputed from scipy's own query (knn.cu: idw_fix_kernel,
 // tree built on a side stream while this kernel runs).  The fill is then the reference's at every
 // grid point (<= 1e-12; the weights use rsqrt where NumPy uses sqrt/power/divide).
+//
+// The search comes in four forms (32-bit keys, packed or unpacked 64-bit keys, an insertion list);
+// idw_fill_kernel is the one rule that chooses among them, for b200_idw_fill and for the device plan
+// of b200_idw_fill_planned alike, and idw_run the fill both entry points share.
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -41,31 +45,44 @@ struct IDWParams {
     double *out;  // (nvar, ny, nx)
     double2 *twin;   // (ny, nx) pairs of the two variables, written beside `out` (or null; nvar == 2 only)
     const B200IdwPlan *plan;  // device plan of b200_idw_fill_planned (or null: the host chose the kernel)
-    int *tie_list;   // grid points whose k-th and (k+1)-th neighbours are equidistant (or null)
+    int *tie_list;   // grid points whose k-th and (k+1)-th neighbours are equidistant
     int *tie_count;
     uint8_t *tile_done;  // per pixel tile: filled by the 32-bit-key kernel (or null)
 };
 
-// With a device plan several fill kernels are enqueued and each decides from the plan whether the
-// field is its own -- the choice the host makes from known counts in b200_idw_fill:
-//   KEY32   idw32_kernel<20>:           k_eff == 20, half-pixel grid, <= IDW_CHUNK vectors
-//   PACKED  idw_kernel<20, true, true>: k_eff == 20, 1/16 grid, <= IDW_CHUNK vectors (tiles KEY32 left)
-//   EXACT   idw_strided_kernel<20, true, false>: k_eff == 20 otherwise
-//   INSERT  idw_strided_kernel<32, false, ...>: k_eff != 20 (the K = 8 network of the host path gives the
-//           same bits: same list, same NumPy-order epilogue)
-// k_eff = min(k, npts).  npts is the plan's n_fill: 0 when the field is constant, zero or refused.
-enum { ROLE_KEY32, ROLE_PACKED, ROLE_EXACT, ROLE_INSERT };
+// dense_lucaskanade's weighting (two variables, power 1/2, unit resolution, positive offset): the
+// weights come from rsqrt instead of NumPy's sqrt, power and divide
+__host__ __device__ __forceinline__ bool fast_weights(const IDWParams &p) {
+    return p.nvar == 2 && p.power == 0.5 && p.mean_res == 1.0 && p.offset > 0.0;
+}
 
-__device__ __forceinline__ bool plan_takes(const B200IdwPlan &pl, int k, int role) {
-    const int n = pl.n_fill;
-    if (n < 1) return false;
-    const bool k20 = min(k, n) == 20, pk = pl.on_grid >= 1 && n <= IDW_CHUNK;
-    switch (role) {
-        case ROLE_KEY32: return k20 && pk && pl.on_grid == 2;
-        case ROLE_PACKED: return k20 && pk;
-        case ROLE_EXACT: return k20 && !pk;
-        default: return !k20;
-    }
+// Which kernel fills the field, for k neighbours among n vectors with key level `level`
+// (coords_on_16th_grid: 2 half-pixel vectors on an integer grid, 1 every coordinate a multiple of 1/16
+// below 2^14, 0 otherwise) and fast weights or not:
+//   KEY32     k == 20 <= n <= IDW_CHUNK, level 2, fast weights: idw32_kernel<20>, then the PACKED
+//             kernel over the tiles whose search radius the 32-bit keys do not hold
+//   PACKED    k == 20 <= n <= IDW_CHUNK, level >= 1: idw_kernel<20, true, true, fastw>
+//   UNPACKED  k == 20 <= n otherwise: idw_kernel<20, true, false, fastw>
+//   INSERT    k != 20 or n < 20: idw_kernel<32, false, false, false>, the insertion list
+//   NONE      n == 0: a device plan whose field is constant, zero or refused
+// b200_idw_fill applies it to the counts it knows; a count on the device takes INSERT.  With a device
+// plan every kernel the rule may pick is enqueued, and each applies it to the plan's n_fill with
+// k = min(k, n_fill) to decide whether the field is its own.
+enum IdwFill { IDW_NONE, IDW_KEY32, IDW_PACKED, IDW_UNPACKED, IDW_INSERT };
+
+__host__ __device__ __forceinline__ IdwFill idw_fill_kernel(int k, int n, int level, bool fastw) {
+    if (n < 1) return IDW_NONE;
+    if (k != 20 || n < k) return IDW_INSERT;
+    if (level == 0 || n > IDW_CHUNK) return IDW_UNPACKED;
+    return (level == 2 && fastw) ? IDW_KEY32 : IDW_PACKED;
+}
+
+// with a device plan: the rule gives the field to another kernel than `mine`
+__device__ __forceinline__ bool plan_declines(const IDWParams &p, IdwFill mine) {
+    if (!p.plan) return false;
+    const int n = p.plan->n_fill;
+    const IdwFill f = idw_fill_kernel(min(p.k, n), n, p.plan->on_grid, fast_weights(p));
+    return !(f == mine || (f == IDW_KEY32 && mine == IDW_PACKED));
 }
 
 // numpy's pairwise summation for n < 128 (8 accumulators, then the remainder)
@@ -104,13 +121,12 @@ __device__ __forceinline__ double np_sum(const double (&w)[K], int k) {
 // without touching the sorted list.  Order of examination is irrelevant for the result:
 // the list is ordered by (squared distance, index), i.e. equal distances resolve to the
 // lower index exactly as cKDTree-free exhaustive scanning in index order would.
-// Batcher odd-even merge sorting networks (generated, verified exhaustively with the 0-1
-// principle): compile-time comparator lists, so the sorted list never leaves registers.
+// Batcher odd-even merge sorting network of 20 (generated, verified exhaustively with the 0-1
+// principle): a compile-time comparator list, so the sorted list never leaves registers.
 __device__ constexpr int NET20[103][2] = {{0,1},{2,3},{4,5},{6,7},{8,9},{10,11},{12,13},{14,15},{16,17},{18,19},{0,2},{1,3},{4,6},{5,7},{8,10},{9,11},{12,14},{13,15},{16,18},{17,19},{1,2},{5,6},{9,10},{13,14},{17,18},{0,4},{1,5},{2,6},{3,7},{8,12},{9,13},{10,14},{11,15},{2,4},{3,5},{10,12},{11,13},{1,2},{3,4},{5,6},{9,10},{11,12},{13,14},{17,18},{0,8},{1,9},{2,10},{3,11},{4,12},{5,13},{6,14},{7,15},{4,8},{5,9},{6,10},{7,11},{2,4},{3,5},{6,8},{7,9},{10,12},{11,13},{1,2},{3,4},{5,6},{7,8},{9,10},{11,12},{13,14},{17,18},{0,16},{1,17},{2,18},{3,19},{8,16},{9,17},{10,18},{11,19},{4,8},{5,9},{6,10},{7,11},{12,16},{13,17},{14,18},{15,19},{2,4},{3,5},{6,8},{7,9},{10,12},{11,13},{14,16},{15,17},{1,2},{3,4},{5,6},{7,8},{9,10},{11,12},{13,14},{15,16},{17,18}};
-__device__ constexpr int NET8[19][2] = {{0,1},{2,3},{4,5},{6,7},{0,2},{1,3},{4,6},{5,7},{1,2},{5,6},{0,4},{1,5},{2,6},{3,7},{2,4},{3,5},{1,2},{3,4},{5,6}};
-template <int K> __device__ __forceinline__ constexpr int net_size() { return K == 20 ? 103 : (K == 8 ? 19 : 0); }
-template <int K> __device__ __forceinline__ constexpr int net_a(int c) { return K == 20 ? NET20[c < 103 ? c : 0][0] : (K == 8 ? NET8[c < 19 ? c : 0][0] : 0); }
-template <int K> __device__ __forceinline__ constexpr int net_b(int c) { return K == 20 ? NET20[c < 103 ? c : 0][1] : (K == 8 ? NET8[c < 19 ? c : 0][1] : 0); }
+template <int K> __device__ __forceinline__ constexpr int net_size() { return K == 20 ? 103 : 0; }
+template <int K> __device__ __forceinline__ constexpr int net_a(int c) { return K == 20 ? NET20[c < 103 ? c : 0][0] : 0; }
+template <int K> __device__ __forceinline__ constexpr int net_b(int c) { return K == 20 ? NET20[c < 103 ? c : 0][1] : 0; }
 
 __device__ __forceinline__ bool key_less(unsigned long long da, int ia, unsigned long long db, int ib) {
     return da < db || (da == db && ia < ib);
@@ -287,8 +303,47 @@ __device__ __forceinline__ TileBound tile_bound(const IDWParams &p, const double
     return tb;
 }
 
-// FASTW: the weighting of dense_lucaskanade's call (two variables, power 1/2, unit resolution,
-// positive offset) from rsqrt; otherwise the general NumPy-order epilogue.
+// Lists grid point g of every lane whose `tie` is set: one atomicAdd per warp, stores compacted.
+__device__ __forceinline__ void tie_append(const IDWParams &p, bool tie, int g) {
+    const int lane = threadIdx.x & 31;
+    const unsigned bal = __ballot_sync(0xffffffffu, tie);
+    if (bal) {
+        int base = 0;
+        if (lane == __ffs(bal) - 1) base = atomicAdd(p.tie_count, __popc(bal));
+        base = __shfl_sync(0xffffffffu, base, __ffs(bal) - 1);
+        if (tie) p.tie_list[base + __popc(bal & ((1u << lane) - 1u))] = g;
+    }
+}
+
+// The fast weighting (fast_weights) of grid point (i, j) over list entries q < k, entry(q, d2, id)
+// giving the squared distance and vector index of each: w = (sqrt(d2) + offset)^-1/2 from two rsqrt
+// (FMA pipe) instead of sqrt, pow and a divide per neighbour, normalised once -- relative error a few
+// 1e-16.  Stores the planar field and its twin.
+template <int K, typename Entry>
+__device__ __forceinline__ void fast_weights_store(const IDWParams &p, int k, int i, int j, Entry entry) {
+    double ws = 0.0, ax = 0.0, ay = 0.0;
+    const double2 *__restrict__ v2 = reinterpret_cast<const double2 *>(p.vals);
+#pragma unroll
+    for (int q = 0; q < K; q++) {
+        if (q < k) {
+            double d2;
+            int id;
+            entry(q, d2, id);
+            const double dist = d2 > 0.0 ? d2 * rsqrt(d2) : 0.0;
+            const double w = rsqrt(dist + p.offset);
+            const double2 v = v2[id];
+            ws += w;
+            ax = fma(w, v.x, ax);
+            ay = fma(w, v.y, ay);
+        }
+    }
+    const double inv = 1.0 / ws, fx = ax * inv, fy = ay * inv;
+    p.out[((size_t)0 * p.ny + i) * p.nx + j] = fx;
+    p.out[((size_t)1 * p.ny + i) * p.nx + j] = fy;
+    if (p.twin) p.twin[(size_t)i * p.nx + j] = make_double2(fx, fy);
+}
+
+// FASTW: the fast weighting; otherwise the general NumPy-order epilogue.
 // One pixel tile (bx, by) of idw_kernel.
 template <int K, bool EXACT, bool PACKED, bool FASTW>
 __device__ __forceinline__ void idw_tile(const IDWParams &p, int bx, int by, int tiles_x) {
@@ -348,7 +403,7 @@ __device__ __forceinline__ void idw_tile(const IDWParams &p, int bx, int by, int
         if (active) topk_scan<K, EXACT, PACKED>(spt, sidx, cnt, qx, qy, k, r == 0, bd, bi, rej);
     }
     // ---- equidistant k-th / (k+1)-th neighbour: listed for the exact-order recomputation -----
-    if (p.tie_list != nullptr) {
+    {
         unsigned long long kth = bd[K - 1];
         if (!EXACT) {
 #pragma unroll
@@ -356,39 +411,14 @@ __device__ __forceinline__ void idw_tile(const IDWParams &p, int bx, int by, int
                 if (q == k - 1) kth = bd[q];
         }
         const unsigned long long dmask = PACKED ? ~2047ull : ~0ull;
-        const bool tie = active && k >= 1 && ((kth & dmask) == (rej & dmask));
-        const unsigned bal = __ballot_sync(0xffffffffu, tie);
-        if (bal) {
-            int base = 0;
-            if (lane == __ffs(bal) - 1) base = atomicAdd(p.tie_count, __popc(bal));
-            base = __shfl_sync(0xffffffffu, base, __ffs(bal) - 1);
-            if (tie) p.tie_list[base + __popc(bal & ((1u << lane) - 1u))] = i * p.nx + j;
-        }
+        tie_append(p, active && k >= 1 && ((kth & dmask) == (rej & dmask)), i * p.nx + j);
     }
     if (!active || k < 1) return;
     if (FASTW) {
-        // dense_lucaskanade's call: w = (sqrt(d2) + offset)^-1/2 from two rsqrt (FMA pipe) instead
-        // of sqrt, pow and a divide per neighbour, normalised once -- relative error a few 1e-16
-        double ws = 0.0, ax = 0.0, ay = 0.0;
-        const double2 *__restrict__ v2 = reinterpret_cast<const double2 *>(p.vals);
-#pragma unroll
-        for (int q = 0; q < K; q++) {
-            if (q < k) {
-                const unsigned long long b = PACKED ? (bd[q] & ~2047ull) : bd[q];
-                const int id = PACKED ? (int)(bd[q] & 2047ull) : bi[q];
-                const double d2 = __longlong_as_double((long long)b);
-                const double dist = d2 > 0.0 ? d2 * rsqrt(d2) : 0.0;
-                const double w = rsqrt(dist + p.offset);
-                const double2 v = v2[id];
-                ws += w;
-                ax = fma(w, v.x, ax);
-                ay = fma(w, v.y, ay);
-            }
-        }
-        const double inv = 1.0 / ws, fx = ax * inv, fy = ay * inv;
-        p.out[((size_t)0 * p.ny + i) * p.nx + j] = fx;
-        p.out[((size_t)1 * p.ny + i) * p.nx + j] = fy;
-        if (p.twin) p.twin[(size_t)i * p.nx + j] = make_double2(fx, fy);
+        fast_weights_store<K>(p, k, i, j, [&](int q, double &d2, int &id) {
+            d2 = __longlong_as_double((long long)(PACKED ? (bd[q] & ~2047ull) : bd[q]));
+            id = PACKED ? (int)(bd[q] & 2047ull) : bi[q];
+        });
         return;
     }
     double w[K];
@@ -418,18 +448,12 @@ __device__ __forceinline__ void idw_tile(const IDWParams &p, int bx, int by, int
     }
 }
 
-// one tile per CTA
+// Every CTA walks the tiles in steps of the grid size.  A grid of one CTA per tile fills each tile at
+// once; the kernels a device plan rarely chooses run on one wave of resident CTAs (resident_grid), so
+// that declining costs one wave instead of one per tile.
 template <int K, bool EXACT, bool PACKED, bool FASTW>
 __global__ void __launch_bounds__(IDW_THREADS, FASTW ? 3 : 1) idw_kernel(const IDWParams p) {
-    if (p.plan && !plan_takes(*p.plan, p.k, EXACT ? (PACKED ? ROLE_PACKED : ROLE_EXACT) : ROLE_INSERT)) return;
-    idw_tile<K, EXACT, PACKED, FASTW>(p, blockIdx.x, blockIdx.y, gridDim.x);
-}
-
-// every CTA walks the tiles in steps of the grid size: b200_idw_fill_planned launches the kernels a plan
-// rarely chooses on one wave of resident CTAs, so that declining costs one wave instead of one per tile
-template <int K, bool EXACT, bool PACKED, bool FASTW>
-__global__ void __launch_bounds__(IDW_THREADS, FASTW ? 3 : 1) idw_strided_kernel(const IDWParams p) {
-    if (p.plan && !plan_takes(*p.plan, p.k, EXACT ? (PACKED ? ROLE_PACKED : ROLE_EXACT) : ROLE_INSERT)) return;
+    if (plan_declines(p, EXACT ? (PACKED ? IDW_PACKED : IDW_UNPACKED) : IDW_INSERT)) return;
     const int tiles_x = (p.nx + IDW_TX - 1) / IDW_TX, ntiles = tiles_x * ((p.ny + IDW_TY - 1) / IDW_TY);
     for (int t = blockIdx.y * gridDim.x + blockIdx.x; t < ntiles; t += gridDim.x * gridDim.y) {
         idw_tile<K, EXACT, PACKED, FASTW>(p, t % tiles_x, t / tiles_x, tiles_x);
@@ -464,7 +488,7 @@ __global__ void __launch_bounds__(IDW_THREADS, 4) idw32_kernel(const IDWParams p
     __shared__ int fill[IDW_BINS];
     __shared__ unsigned char sbin[IDW_CHUNK];
     __shared__ int s_bmax, s_total;
-    if (p.plan && !plan_takes(*p.plan, p.k, ROLE_KEY32)) return;
+    if (plan_declines(p, IDW_KEY32)) return;
     const int npts = p.npts_dev ? min(*p.npts_dev, p.npts_cap) : p.npts_cap;
     const int k = K;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -519,34 +543,13 @@ __global__ void __launch_bounds__(IDW_THREADS, 4) idw32_kernel(const IDWParams p
             }
         }
     }
-    if (p.tie_list != nullptr) {
-        const bool tie = active && ((bd[K - 1] >> 11) == (rej >> 11));
-        const unsigned bal = __ballot_sync(0xffffffffu, tie);
-        if (bal) {
-            int base = 0;
-            if (lane == __ffs(bal) - 1) base = atomicAdd(p.tie_count, __popc(bal));
-            base = __shfl_sync(0xffffffffu, base, __ffs(bal) - 1);
-            if (tie) p.tie_list[base + __popc(bal & ((1u << lane) - 1u))] = i * p.nx + j;
-        }
-    }
+    tie_append(p, active && ((bd[K - 1] >> 11) == (rej >> 11)), i * p.nx + j);
     if (tid == 0) p.tile_done[blockIdx.y * gridDim.x + blockIdx.x] = 1;
     if (!active) return;
-    double ws = 0.0, ax = 0.0, ay = 0.0;
-    const double2 *__restrict__ v2 = reinterpret_cast<const double2 *>(p.vals);
-#pragma unroll
-    for (int q = 0; q < K; q++) {
-        const double d2 = (double)(bd[q] >> 11) * 0.25;
-        const double dist = d2 > 0.0 ? d2 * rsqrt(d2) : 0.0;
-        const double w = rsqrt(dist + p.offset);
-        const double2 v = v2[bd[q] & 2047u];
-        ws += w;
-        ax = fma(w, v.x, ax);
-        ay = fma(w, v.y, ay);
-    }
-    const double inv = 1.0 / ws, fx = ax * inv, fy = ay * inv;
-    p.out[((size_t)0 * p.ny + i) * p.nx + j] = fx;
-    p.out[((size_t)1 * p.ny + i) * p.nx + j] = fy;
-    if (p.twin) p.twin[(size_t)i * p.nx + j] = make_double2(fx, fy);
+    fast_weights_store<K>(p, K, i, j, [&](int q, double &d2, int &id) {
+        d2 = (double)(bd[q] >> 11) * 0.25;
+        id = (int)(bd[q] & 2047u);
+    });
 }
 
 // ---- device plan (b200_idw_plan) -----------------------------------------------------------------
@@ -675,6 +678,75 @@ int side_stream(SideStream **out) {
     return 0;
 }
 
+template <typename F>
+void launch_tiles(F kernel, const IDWParams &p, dim3 grid, bool resident, cudaStream_t s) {
+    kernel<<<resident ? resident_grid(kernel, grid) : grid, IDW_THREADS, 0, s>>>(p);
+}
+
+// Enqueues the kernel(s) of fill f (see idw_fill_kernel) on the full tile grid, or on one wave of
+// resident CTAs.
+int launch_fill(IdwFill f, IDWParams p, bool resident, b200::Scratch &done, cudaStream_t s) {
+    const dim3 grid(b200::ceil_div(p.nx, IDW_TX), b200::ceil_div(p.ny, IDW_TY));
+    const bool fastw = fast_weights(p);
+    if (f == IDW_KEY32) {
+        const size_t ntiles = (size_t)grid.x * grid.y;
+        B200_CUDA(done.alloc(ntiles, s));
+        B200_CUDA(cudaMemsetAsync(done.p, 0, ntiles, s));
+        p.tile_done = (uint8_t *)done.p;
+        idw32_kernel<20><<<grid, IDW_THREADS, 0, s>>>(p);
+        B200_LAUNCH_CHECK();
+        f = IDW_PACKED;  // over the tiles idw32_kernel leaves
+    }
+    if (f == IDW_PACKED && fastw) launch_tiles(idw_kernel<20, true, true, true>, p, grid, resident, s);
+    else if (f == IDW_PACKED) launch_tiles(idw_kernel<20, true, true, false>, p, grid, resident, s);
+    else if (f == IDW_UNPACKED && fastw) launch_tiles(idw_kernel<20, true, false, true>, p, grid, resident, s);
+    else if (f == IDW_UNPACKED) launch_tiles(idw_kernel<20, true, false, false>, p, grid, resident, s);
+    else launch_tiles(idw_kernel<32, false, false, false>, p, grid, resident, s);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+// The fill of both entry points for the p.npts_dev (or p.npts_cap) vectors: the cKDTree of the vectors on
+// the side stream (see the header comment) while the fill kernels run on `s`, then the recomputation of
+// the listed grid points.  Without a device plan the rule picks one fill from the key level `level`.  With
+// one (p.plan) the plan's constant field is written first, and every fill the rule may pick is enqueued:
+// the plan's usual choice on the full tile grid, the rare ones on one wave of resident CTAs.
+int idw_run(IDWParams p, int level, cudaStream_t s) {
+    const size_t N = (size_t)p.ny * p.nx;
+    B200_REQUIRE(N < ((size_t)1 << 31), "grid too large");
+    if (p.plan) {
+        const int blocks = (int)std::max<size_t>(1, std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 8));
+        idw_plan_const_kernel<<<blocks, 256, 0, s>>>(p.plan, p.out, p.twin, N);
+        B200_LAUNCH_CHECK();
+    }
+    kdp::TreeScratch ts;
+    b200::Scratch tie, done;
+    SideStream *ss = nullptr;
+    if (int rc = side_stream(&ss)) return rc;
+    if (int rc = kdp::tree_alloc(ts, p.npts_cap, s)) return rc;
+    B200_CUDA(tie.alloc(sizeof(int) * (N + 1), s));
+    p.tie_count = (int *)tie.p;
+    p.tie_list = p.tie_count + 1;
+    B200_CUDA(cudaMemsetAsync(p.tie_count, 0, sizeof(int), s));
+    B200_CUDA(cudaEventRecord(ss->fork, s));
+    B200_CUDA(cudaStreamWaitEvent(ss->s, ss->fork, 0));
+    if (int rc = kdp::tree_build(p.xy, p.npts_dev, p.npts_cap, ts.tb, ss->s)) return rc;
+    B200_CUDA(cudaEventRecord(ss->join, ss->s));
+    if (!p.plan) {
+        const IdwFill f = p.npts_dev ? IDW_INSERT : idw_fill_kernel(p.k, p.npts_cap, level, fast_weights(p));
+        if (int rc = launch_fill(f, p, false, done, s)) return rc;
+    } else {
+        if (p.k >= 20) {  // min(k, n_fill) can be 20
+            if (int rc = launch_fill(fast_weights(p) ? IDW_KEY32 : IDW_PACKED, p, false, done, s)) return rc;
+            if (int rc = launch_fill(IDW_UNPACKED, p, true, done, s)) return rc;
+        }
+        if (int rc = launch_fill(IDW_INSERT, p, true, done, s)) return rc;
+    }
+    B200_CUDA(cudaStreamWaitEvent(s, ss->join, 0));
+    return kdp::idw_fix(p.xy, p.vals, p.nvar, p.k, p.power, p.offset, p.mean_res, p.gx, p.nx, p.gy, p.ny, ts.tb,
+                        p.tie_list, p.tie_count, p.out, p.twin, s);
+}
+
 }  // namespace
 
 extern "C" int b200_idw_fill(const double *xy, const double *vals, const int *npts_dev, int npts_cap,
@@ -687,60 +759,13 @@ extern "C" int b200_idw_fill(const double *xy, const double *vals, const int *np
         b200::set_error("idw: k must be <= 32 (k=None / larger k is not implemented)");
         return B200_ENOTSUP;
     }
-    cudaStream_t s = (cudaStream_t)stream;
-    // ---- cKDTree of the vectors on the side stream (see the header comment) -----------------
-    kdp::TreeScratch ts;
-    b200::Scratch tie;
-    SideStream *ss = nullptr;
-    if (int rc = side_stream(&ss)) return rc;
-    if (int rc = kdp::tree_alloc(ts, npts_cap, s)) return rc;
-    const size_t N = (size_t)ny * nx;
-    B200_REQUIRE(N < ((size_t)1 << 31), "grid too large");
-    B200_CUDA(tie.alloc(sizeof(int) * (N + 1), s));
-    int *tie_count = (int *)tie.p, *tie_list = tie_count + 1;
-    B200_CUDA(cudaMemsetAsync(tie_count, 0, sizeof(int), s));
-    B200_CUDA(cudaEventRecord(ss->fork, s));
-    B200_CUDA(cudaStreamWaitEvent(ss->s, ss->fork, 0));
-    if (int rc = kdp::tree_build(xy, npts_dev, npts_cap, ts.tb, ss->s)) return rc;
-    B200_CUDA(cudaEventRecord(ss->join, ss->s));
-
-    IDWParams p;
+    IDWParams p = {};
     p.xy = xy; p.vals = vals; p.npts_dev = npts_dev; p.npts_cap = npts_cap; p.nvar = nvar; p.k = k;
     p.gx = xgrid; p.gy = ygrid; p.nx = nx; p.ny = ny;
     p.power = power; p.offset = dist_offset; p.mean_res = mean_res; p.out = out;
-    p.tie_list = tie_list; p.tie_count = tie_count;
-    p.tile_done = nullptr;
-    p.twin = nullptr;
-    p.plan = nullptr;
-    dim3 grid(b200::ceil_div(nx, IDW_TX), b200::ceil_div(ny, IDW_TY));
-    dim3 block(IDW_THREADS);
-    // the host knows npts only as a capacity when npts_dev is given; EXACT needs k == K <= npts
-    const bool exact_ok = (npts_dev == nullptr) && npts_cap >= k;
-    // the caller vouches that every coordinate (vectors and grid) is a multiple of 1/16 with
-    // magnitude < 2^14; with <= 2048 vectors the index fits the zero low bits of the distance
-    const bool packed = coords_on_16th_grid != 0 && exact_ok && npts_cap <= IDW_CHUNK;
-    const bool fastw = nvar == 2 && power == 0.5 && mean_res == 1.0 && dist_offset > 0.0;
-    b200::Scratch done;
-    if (k == 20 && packed && fastw && coords_on_16th_grid == 2) {
-        // vectors on the half-pixel grid, grid on integers: 32-bit integer keys wherever the search
-        // radius allows, the 64-bit kernel behind it for the tiles it left
-        const size_t ntiles = (size_t)grid.x * grid.y;
-        B200_CUDA(done.alloc(ntiles, s));
-        B200_CUDA(cudaMemsetAsync(done.p, 0, ntiles, s));
-        p.tile_done = (uint8_t *)done.p;
-        idw32_kernel<20><<<grid, block, 0, s>>>(p);
-        B200_LAUNCH_CHECK();
-    }
-    if (k == 20 && packed && fastw) idw_kernel<20, true, true, true><<<grid, block, 0, s>>>(p);
-    else if (k == 20 && packed) idw_kernel<20, true, true, false><<<grid, block, 0, s>>>(p);
-    else if (k == 20 && exact_ok && fastw) idw_kernel<20, true, false, true><<<grid, block, 0, s>>>(p);
-    else if (k == 20 && exact_ok) idw_kernel<20, true, false, false><<<grid, block, 0, s>>>(p);
-    else if (k == 8 && exact_ok) idw_kernel<8, true, false, false><<<grid, block, 0, s>>>(p);
-    else idw_kernel<32, false, false, false><<<grid, block, 0, s>>>(p);
-    B200_LAUNCH_CHECK();
-    B200_CUDA(cudaStreamWaitEvent(s, ss->join, 0));
-    return kdp::idw_fix(xy, vals, nvar, k, power, dist_offset, mean_res, xgrid, nx, ygrid, ny, ts.tb, tie_list,
-                        tie_count, out, nullptr, s);
+    // the caller vouches for the key level: every coordinate (vectors and grid) a multiple of 1/16
+    // below 2^14, and with 2 also the vectors on the half-pixel grid and the grid on integers
+    return idw_run(p, coords_on_16th_grid, (cudaStream_t)stream);
 }
 
 extern "C" int b200_idw_plan(const int *counts, const double *xy, const double *uv, int cap, int grid_ok,
@@ -751,10 +776,11 @@ extern "C" int b200_idw_plan(const int *counts, const double *xy, const double *
     return 0;
 }
 
-// b200_idw_fill with the vector count and the path taken from a device plan: every kernel that may
-// fill the field is enqueued (grids and scratch sized from the capacity) and all but the one the plan
-// chooses return at once (see plan_takes).  The path the plan chooses is the one b200_idw_fill takes
-// for the same vectors, so the field is the same bit for bit.
+// b200_idw_fill with the vector count, the key level and the early-outs taken from a device plan: every
+// kernel that may fill the field is enqueued (grids and scratch sized from the capacity) and each returns
+// at once unless the rule of b200_idw_fill, applied to the plan, gives it the field; the zero and
+// constant fields are written by idw_plan_const_kernel.  The field is therefore b200_idw_fill's for the
+// same vectors, bit for bit.
 extern "C" int b200_idw_fill_planned(const double *xy, const double *vals, const B200IdwPlan *plan, int npts_cap,
                                      int k, double power, double dist_offset, const double *xgrid, int nx,
                                      const double *ygrid, int ny, double *out, double *twin, void *stream) {
@@ -764,65 +790,12 @@ extern "C" int b200_idw_fill_planned(const double *xy, const double *vals, const
         b200::set_error("idw: k must be <= 32 (k=None / larger k is not implemented)");
         return B200_ENOTSUP;
     }
-    cudaStream_t s = (cudaStream_t)stream;
-    const size_t N = (size_t)ny * nx;
-    B200_REQUIRE(N < ((size_t)1 << 31), "grid too large");
-    {
-        const int blocks = (int)std::max<size_t>(1, std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 8));
-        idw_plan_const_kernel<<<blocks, 256, 0, s>>>(plan, out, (double2 *)twin, N);
-        B200_LAUNCH_CHECK();
-    }
-    kdp::TreeScratch ts;
-    b200::Scratch tie, done;
-    SideStream *ss = nullptr;
-    if (int rc = side_stream(&ss)) return rc;
-    if (int rc = kdp::tree_alloc(ts, npts_cap, s)) return rc;
-    B200_CUDA(tie.alloc(sizeof(int) * (N + 1), s));
-    int *tie_count = (int *)tie.p, *tie_list = tie_count + 1;
-    B200_CUDA(cudaMemsetAsync(tie_count, 0, sizeof(int), s));
-    B200_CUDA(cudaEventRecord(ss->fork, s));
-    B200_CUDA(cudaStreamWaitEvent(ss->s, ss->fork, 0));
-    // a tree of the n_fill vectors: empty unless the plan interpolates
-    if (int rc = kdp::tree_build(xy, &plan->n_fill, npts_cap, ts.tb, ss->s)) return rc;
-    B200_CUDA(cudaEventRecord(ss->join, ss->s));
-
-    IDWParams p;
-    memset(&p, 0, sizeof(p));
+    IDWParams p = {};
     p.xy = xy; p.vals = vals; p.npts_dev = &plan->n_fill; p.npts_cap = npts_cap; p.nvar = 2; p.k = k;
     p.gx = xgrid; p.gy = ygrid; p.nx = nx; p.ny = ny;
     p.power = power; p.offset = dist_offset; p.mean_res = 1.0; p.out = out; p.twin = (double2 *)twin;
     p.plan = plan;
-    p.tie_list = tie_list; p.tie_count = tie_count;
-    dim3 grid(b200::ceil_div(nx, IDW_TX), b200::ceil_div(ny, IDW_TY));
-    dim3 block(IDW_THREADS);
-    const bool fastw = power == 0.5 && dist_offset > 0.0;
-    if (k >= 20) {  // k_eff = min(k, n) can be 20: the register-resident K = 20 kernels
-        if (fastw) {
-            const size_t ntiles = (size_t)grid.x * grid.y;
-            B200_CUDA(done.alloc(ntiles, s));
-            B200_CUDA(cudaMemsetAsync(done.p, 0, ntiles, s));
-            p.tile_done = (uint8_t *)done.p;
-            idw32_kernel<20><<<grid, block, 0, s>>>(p);
-            B200_LAUNCH_CHECK();
-            idw_kernel<20, true, true, true><<<grid, block, 0, s>>>(p);
-            B200_LAUNCH_CHECK();
-            p.tile_done = nullptr;
-            auto *kx = idw_strided_kernel<20, true, false, true>;
-            kx<<<resident_grid(kx, grid), block, 0, s>>>(p);
-        } else {
-            idw_kernel<20, true, true, false><<<grid, block, 0, s>>>(p);
-            B200_LAUNCH_CHECK();
-            auto *kx = idw_strided_kernel<20, true, false, false>;
-            kx<<<resident_grid(kx, grid), block, 0, s>>>(p);
-        }
-        B200_LAUNCH_CHECK();
-    }
-    auto *ki = idw_strided_kernel<32, false, false, false>;
-    ki<<<resident_grid(ki, grid), block, 0, s>>>(p);
-    B200_LAUNCH_CHECK();
-    B200_CUDA(cudaStreamWaitEvent(s, ss->join, 0));
-    return kdp::idw_fix(xy, vals, 2, k, power, dist_offset, 1.0, xgrid, nx, ygrid, ny, ts.tb, tie_list,
-                        tie_count, out, (double2 *)twin, s);
+    return idw_run(p, 0, (cudaStream_t)stream);  // the plan holds the key level
 }
 
 extern "C" int b200_idw_fill_all(const double *xy, const double *vals, const int *npts_dev, int npts_cap, int nvar,

@@ -224,6 +224,46 @@ def _attach_twin(out, twin, interp_kwargs):
     out._b200_twin_version = out._version
 
 
+# ---- the host-side tail of the interpolation, shared with stages.idwinterp2d -------------------------
+def _idw_constant(out, v2):
+    """decorators.py:200-208: the constant field of one vector, or of (n, nvar) values that are all equal,
+    into the (nvar, ny, nx) device tensor `out`.  Returns whether the field was constant."""
+    if v2.shape[0] == 1:
+        for c in range(v2.shape[1]):
+            _call("b200_fill_f64", out[c].data_ptr(), out[c].numel(), float(1.0 * v2[0, c]), _s())
+        return True
+    if v2.max() == v2.min():
+        _call("b200_fill_f64", out.data_ptr(), out.numel(), float(1.0 * v2.ravel()[0]), _s())
+        return True
+    return False
+
+
+def _key_level(xy_h, grid_level):
+    """coords_on_16th_grid of b200_idw_fill: 1 when every coordinate is a multiple of 1/16 below 2^14 (squared
+    distances are exact multiples of 1/256: packed 64-bit keys), 2 when moreover the vectors sit on the
+    half-pixel grid (medians of integer corners) and the grid on integers (32-bit keys), else 0.  grid_level()
+    is the grid's own level, asked only when the vectors qualify."""
+    if not (np.all(xy_h * 16.0 == np.rint(xy_h * 16.0)) and np.abs(xy_h).max() < 16384.0):
+        return 0
+    g = grid_level()
+    if not g:
+        return 0
+    return 2 if g == 2 and np.all(xy_h * 2.0 == np.rint(xy_h * 2.0)) else 1
+
+
+def _idw_fill(dxy, dv, npts, nvar, k, power, dist_offset, mean_res, gx, nx, gy, ny, level, out):
+    """Fills `out` (nvar, ny, nx) from npts device vectors: exhaustive tile search, grid points whose neighbour
+    set depends on cKDTree's tie order recomputed from its query (csrc/idw.cu, knn.cu); k=None: every vector
+    weighs in at every grid point (interpolate.py:82-88)."""
+    if k is None:
+        _call("b200_idw_fill_all", dxy.data_ptr(), dv.data_ptr(), None, npts, nvar, float(power),
+              float(dist_offset), mean_res, gx.data_ptr(), nx, gy.data_ptr(), ny, out.data_ptr(), _s())
+    else:
+        _call("b200_idw_fill", dxy.data_ptr(), dv.data_ptr(), None, npts, nvar, int(min(int(k), npts)),
+              float(power), float(dist_offset), mean_res, gx.data_ptr(), nx, gy.data_ptr(), ny, int(level),
+              out.data_ptr(), _s())
+
+
 def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kwargs=None,
                       interp_method="idwinterp2d", interp_kwargs=None, dense=True,
                       nr_std_outlier=3, k_outlier=30, size_opening=3, decl_scale=20,
@@ -499,31 +539,14 @@ def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kw
         raise ValueError("argument 'values' contains non-finite values")
     if np.any(~np.isfinite(xy_h)):
         raise ValueError("argument 'xy_coord' contains non-finite values")
-    if n_dec == 1:  # decorators.py:200-204
-        for c in range(2):
-            _call("b200_fill_f64", out[c].data_ptr(), mb * n, float(1.0 * uv_h[0, c]), _s())
-    elif uv_h.max() == uv_h.min():  # decorators.py:207-208
-        _call("b200_fill_f64", out.data_ptr(), 2 * mb * n, float(1.0 * uv_h.ravel()[0]), _s())
-    else:
+    if not _idw_constant(out, uv_h):
         if n < 2 or m < 2:
             raise ValueError("Shape of array too small to calculate a numerical gradient, "
                              "at least (edge_order + 1) elements are required.")
         xgrid, ygrid = _pixel_grid(0, n), _pixel_grid(r0, r1)
-        # integer pixel grid + corner coordinates that are integers or cell medians (multiples
-        # of 1/2): squared distances are exact small multiples of 1/256 -> packed-key fast path
-        on_grid = int(bool(np.all(xy_h * 16.0 == np.rint(xy_h * 16.0)) and np.abs(xy_h).max() < 16384.0
-                           and max(m, n) < 16384))
-        if on_grid and np.all(xy_h * 2.0 == np.rint(xy_h * 2.0)):
-            on_grid = 2  # half-pixel grid (the usual case: medians of integers): 32-bit integer keys
-        # exhaustive tile search; grid points whose neighbour set depends on cKDTree's tie order are
-        # recomputed from its query (csrc/idw.cu, knn.cu)
-        if k is None:  # every vector weighs in at every grid point (interpolate.py:82-88)
-            _call("b200_idw_fill_all", dec_xy.data_ptr(), dec_uv.data_ptr(), None, n_dec, 2, power, dist_offset, 1.0,
-                  xgrid.data_ptr(), n, ygrid.data_ptr(), mb, out.data_ptr(), _s())
-        else:
-            _call("b200_idw_fill", dec_xy.data_ptr(), dec_uv.data_ptr(), None, n_dec, 2, int(min(int(k), n_dec)),
-                  power, dist_offset, 1.0, xgrid.data_ptr(), n, ygrid.data_ptr(), mb, on_grid,
-                  out.data_ptr(), _s())
+        # the integer pixel grid holds the key level while max(m, n) < 16384
+        level = _key_level(xy_h, lambda: 2 if max(m, n) < 16384 else 0)
+        _idw_fill(dec_xy, dec_uv, n_dec, 2, k, power, dist_offset, 1.0, xgrid, n, ygrid, mb, level, out)
 
     if verbose:
         torch.cuda.current_stream().synchronize()

@@ -235,12 +235,7 @@ def idwinterp2d(xy_coord, values, xgrid, ygrid, power=0.5, k=20, dist_offset=0.5
     out = torch.empty((nvar, ny, nx), dtype=torch.float64, device="cuda")
     v2 = v_h.reshape(v_h.shape[0], nvar)
     npts = v2.shape[0]
-    if npts == 1:  # decorators.py:200-204
-        for c in range(nvar):
-            _lib.call("b200_fill_f64", out[c].data_ptr(), ny * nx, float(1.0 * v2[0, c]), _s())
-    elif v2.max() == v2.min():  # decorators.py:207-208
-        _lib.call("b200_fill_f64", out.data_ptr(), nvar * ny * nx, float(1.0 * v2.ravel()[0]), _s())
-    else:
+    if not _lk._idw_constant(out, v2):
         xg = np.ascontiguousarray(xgrid, dtype=np.float64)
         yg = np.ascontiguousarray(ygrid, dtype=np.float64)
         for g in (xg, yg):
@@ -255,27 +250,21 @@ def idwinterp2d(xy_coord, values, xgrid, ygrid, power=0.5, k=20, dist_offset=0.5
         suby = [y for y in np.array_split(yg, nchunks) if y.size > 0] if nchunks > 1 else [yg]
         res = [[float(np.mean(np.abs([np.gradient(sx).mean(), np.gradient(sy).mean()]))) for sy in suby]
                for sx in subx]
-        on_grid = bool(np.all(xy_h * 16.0 == np.rint(xy_h * 16.0)) and np.abs(xy_h).max() < 16384.0
-                       and np.all(xg * 16.0 == np.rint(xg * 16.0)) and np.all(yg * 16.0 == np.rint(yg * 16.0))
-                       and max(np.abs(xg).max(), np.abs(yg).max()) < 16384.0)
-        on_grid = int(on_grid)
-        if on_grid and np.all(xy_h * 2.0 == np.rint(xy_h * 2.0)) and np.all(xg == np.rint(xg)) \
-                and np.all(yg == np.rint(yg)):
-            on_grid = 2  # half-pixel vectors on an integer grid: 32-bit integer keys (csrc/idw.cu)
+
+        def grid_level():  # the target grid's key level (motion.lucaskanade._key_level)
+            if not (np.all(xg * 16.0 == np.rint(xg * 16.0)) and np.all(yg * 16.0 == np.rint(yg * 16.0))
+                    and max(np.abs(xg).max(), np.abs(yg).max()) < 16384.0):
+                return 0
+            return 2 if np.all(xg == np.rint(xg)) and np.all(yg == np.rint(yg)) else 1
+
+        level = _lk._key_level(xy_h, grid_level)
         dxy = _device.to_device(np.ascontiguousarray(xy_h))
         dv = _device.to_device(np.ascontiguousarray(v2))
-        kk = npts if k is None else int(min(int(k), npts))
 
         def fill(gx, gy, mean_res, dst):
             dgx, dgy = _device.to_device(gx), _device.to_device(gy)
-            if k is None:  # every point weighs in (interpolate.py:82-88)
-                _lib.call("b200_idw_fill_all", dxy.data_ptr(), dv.data_ptr(), None, npts, nvar, float(power),
-                          float(dist_offset), mean_res, dgx.data_ptr(), gx.size, dgy.data_ptr(), gy.size,
-                          dst.data_ptr(), _s())
-                return
-            _lib.call("b200_idw_fill", dxy.data_ptr(), dv.data_ptr(), None, npts, nvar, kk, float(power),
-                      float(dist_offset), mean_res, dgx.data_ptr(), gx.size, dgy.data_ptr(), gy.size,
-                      int(on_grid), dst.data_ptr(), _s())
+            _lk._idw_fill(dxy, dv, npts, nvar, k, power, dist_offset, mean_res, dgx, gx.size, dgy, gy.size, level,
+                          dst)
 
         if len({r for row in res for r in row}) == 1:
             fill(xg, yg, res[0][0], out)

@@ -135,7 +135,7 @@ def test_non_finite_inputs_raise_the_read_back_paths_errors(env, monkeypatch):
     ("general", 300, 20, 0.5, 0.5, 0),    # unpacked 64-bit keys
     ("half", 2500, 20, 0.5, 0.5, 2),      # more vectors than the packed index holds: unpacked
     ("half", 7, 20, 0.5, 0.5, 2),         # fewer vectors than k: insertion list
-    ("half", 100, 8, 0.5, 0.5, 2),        # k = 8 (the read-back path's K = 8 network)
+    ("half", 100, 8, 0.5, 0.5, 2),        # k = 8: the insertion list on both paths
     ("general", 20, 25, 0.5, 0.5, 0),     # k > npts == 20: the K = 20 kernels
     ("half", 100, 25, 0.5, 0.5, 2),       # k = 25
     ("half", 300, 20, 1.5, 0.25, 2),      # general weights
