@@ -1,6 +1,8 @@
 """GPU parity tests of the device cKDTree (csrc/knn.cu): the warp-parallel build gives scipy's
 tree order (oracle/ckdtree.py is pinned against the scipy binary), the outlier stage and the
-grid fill follow its neighbour order at exact distance ties."""
+grid fill follow its neighbour order at exact distance ties.  Branch coverage of the grid fill's tile
+search (every search form, far, partial and multi-round tiles, count and key-level boundaries) lives in
+test_idw_edges_gpu.py."""
 import numpy as np
 import pytest
 
