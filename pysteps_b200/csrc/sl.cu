@@ -32,7 +32,7 @@ struct SLParams {
     double *disp_out;       // (2,m,n) or null
     double *vinc_out;       // (2,m,n) or null
     void *out;              // (T,m,n) planes of this chunk
-    int m, n, T, n_iter, ti_offset, init_mode, mode, has_prev, vel_f32;
+    int m, n, T, n_iter, ti_offset, init_mode, mode, has_prev;
     int row0, rows;         // output band [row0, row0 + rows): band-shaped out / disp arrays
     // batched members (blockIdx.z): element strides between consecutive members, 0 when unused
     size_t zs_vi, zs_precip, zs_disp, zs_out;
@@ -305,11 +305,11 @@ __device__ __forceinline__ void sl_pixel(const SLParams &p, const int x, const i
     }
 }
 
-template <typename F, bool NITER1, int BY, bool VF32, bool BATCH = false>
-__global__ void __launch_bounds__(SL_BX *BY)
+template <typename F, bool NITER1, bool VF32, bool BATCH = false>
+__global__ void __launch_bounds__(SL_BX *SL_BY)
 sl_multistep_kernel(const __grid_constant__ SLParams p) {
     const int x = blockIdx.x * SL_BX + threadIdx.x;
-    const int yl = blockIdx.y * BY + threadIdx.y;  // row inside the band
+    const int yl = blockIdx.y * SL_BY + threadIdx.y;  // row inside the band
     if (x >= p.n || yl >= p.rows) return;
     sl_pixel<F, NITER1, VF32, BATCH, double>(p, x, yl, BATCH ? blockIdx.z : 0);  // z: member of a batched launch
 }
@@ -479,21 +479,22 @@ sl_f32_fixup_kernel(const __grid_constant__ SLParams p, const unsigned *__restri
     if (nfallback && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(nfallback, (unsigned long long)cnt);
 }
 
-// (2,m,n) planar or (m,n,2) interleaved velocity of dtype F -> (m,n) double2
-template <typename F>
+// (2,m,n) planar or (m,n,2) interleaved pairs of type F -> (m,n) pairs of type P2 (rounded to nearest)
+template <typename F, typename P2, bool INTERLEAVED>
 __global__ void __launch_bounds__(256)
-widen_velocity_kernel(const F *__restrict__ V, double2 *__restrict__ Vi, size_t N, int interleaved) {
+relayout_kernel(const F *__restrict__ V, P2 *__restrict__ out, size_t N) {
+    using E = decltype(P2::x);
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += stride) {
-        double2 v;
-        if (interleaved) {
-            v.x = (double)__ldg(V + 2 * i);
-            v.y = (double)__ldg(V + 2 * i + 1);
+        P2 v;
+        if (INTERLEAVED) {
+            v.x = (E)__ldg(V + 2 * i);
+            v.y = (E)__ldg(V + 2 * i + 1);
         } else {
-            v.x = (double)__ldg(V + i);
-            v.y = (double)__ldg(V + N + i);
+            v.x = (E)__ldg(V + i);
+            v.y = (E)__ldg(V + N + i);
         }
-        Vi[i] = v;
+        out[i] = v;
     }
 }
 
@@ -504,254 +505,154 @@ widen_field_kernel(const float *__restrict__ a, double *__restrict__ o, size_t N
         o[i] = (double)__ldg(a + i);
 }
 
-// planar (2,m,n) -> interleaved (m,n,2), same dtype
-template <typename F, typename F2>
-__global__ void __launch_bounds__(256)
-interleave_kernel(const F *__restrict__ V, F2 *__restrict__ Vi, size_t N) {
-    const size_t stride = (size_t)gridDim.x * blockDim.x;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += stride) {
-        F2 v;
-        v.x = __ldg(V + i);
-        v.y = __ldg(V + N + i);
-        Vi[i] = v;
-    }
+// blocks of 256 threads for a grid-stride loop over N elements, at most per_sm of them per SM
+int stream_blocks(size_t N, int per_sm) {
+    return (int)std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * per_sm);
 }
 
-template <typename FV, typename F>
-int sl_run(const void *precip, const void *velocity, const double *xy, const double *disp_prev,
-           const double *tdiff, int T, double vts, int n_iter, double outval, int mode,
-           int layout, int m, int n, int row0, int rows, void *out, double *disp_out,
-           cudaStream_t stream) {
-    const size_t N = (size_t)m * n;          // full frame (inputs)
-    const size_t NB = (size_t)rows * n;      // output band
-    b200::Scratch vi, pw, st_disp, st_vinc;
-    const int sblocks = (int)std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 16);
-    // widen the fields to float64 once (exact), so the trajectory loop issues no conversions
-    const void *vi_ptr = velocity;
-    if (!(sizeof(FV) == 8 && layout == B200_LAYOUT_INTERLEAVED)) {
-        B200_CUDA(vi.alloc(N * sizeof(double2), stream));
-        vi_ptr = vi.p;
-        widen_velocity_kernel<FV><<<sblocks, 256, 0, stream>>>(
-            (const FV *)velocity, (double2 *)vi.p, N, layout == B200_LAYOUT_INTERLEAVED);
-        B200_LAUNCH_CHECK();
+// The velocity as (m,n) pairs of type P2: the caller's buffer when it already is one, otherwise a copy
+// in `buf`, re-laid out and widened (float64 pairs: exact) or rounded (float32 pairs) from type F.
+template <typename P2, typename F>
+int velocity_pairs(const void *velocity, int layout, size_t N, b200::Scratch &buf, const P2 *&pairs,
+                   cudaStream_t stream) {
+    constexpr bool SAME = sizeof(P2) == 2 * sizeof(F);
+    if (SAME && layout == B200_LAYOUT_INTERLEAVED) {
+        pairs = (const P2 *)velocity;
+        return 0;
     }
-    const void *p_ptr = precip;
-    if (precip && sizeof(F) == 4) {
-        B200_CUDA(pw.alloc(N * sizeof(double), stream));
-        p_ptr = pw.p;
-        widen_field_kernel<<<sblocks, 256, 0, stream>>>((const float *)precip, (double *)pw.p, N);
-        B200_LAUNCH_CHECK();
+    B200_CUDA(buf.alloc(N * sizeof(P2), stream));
+    pairs = (const P2 *)buf.p;
+    const int blocks = stream_blocks(N, 16);
+    if (layout == B200_LAYOUT_PLANAR)
+        relayout_kernel<F, P2, false><<<blocks, 256, 0, stream>>>((const F *)velocity, (P2 *)buf.p, N);
+    else if constexpr (!SAME)
+        relayout_kernel<F, P2, true><<<blocks, 256, 0, stream>>>((const F *)velocity, (P2 *)buf.p, N);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+template <typename T> struct Type { using type = T; };
+
+// f(Type<float>{}) or f(Type<double>{}) for a dtype code (the entry points with one dtype take it for a velocity)
+template <typename Fn>
+int with_dtype(int dtype, Fn &&f) {
+    if (dtype == B200_F32) return f(Type<float>{});
+    if (dtype == B200_F64) return f(Type<double>{});
+    b200::set_error("unknown velocity dtype %d", dtype);
+    return B200_EINVAL;
+}
+
+// f(Type<FV>{}, Type<FP>{}) for the dtype codes of a velocity and a precipitation field
+template <typename Fn>
+int with_dtypes(int velocity_dtype, int precip_dtype, Fn &&f) {
+    const auto known = [](int d) { return d == B200_F32 || d == B200_F64; };
+    if (!known(velocity_dtype) || !known(precip_dtype)) {
+        b200::set_error("unknown field dtypes %d / %d", velocity_dtype, precip_dtype);
+        return B200_EINVAL;
     }
-    const int nchunks = (T + SL_MAX_T - 1) / SL_MAX_T;
-    if (nchunks > 1) {
-        B200_CUDA(st_disp.alloc(2 * NB * sizeof(double), stream));
+    return with_dtype(velocity_dtype,
+                      [&](auto fv) { return with_dtype(precip_dtype, [&](auto fp) { return f(fv, fp); }); });
+}
+
+// The argument rules the row-band entry points share, in the order they are checked.  `args_ok` and
+// `args_msg` are the entry point's own rule for its pointer arguments.
+int check_band(int m, int n, int row0, int rows, int layout, bool args_ok, const char *args_msg,
+               const double *tdiff, int T, int n_iter, int mode) {
+    B200_REQUIRE(row0 >= 0 && rows >= 1 && row0 + rows <= m, "row band out of range");
+    B200_REQUIRE(layout == B200_LAYOUT_PLANAR || layout == B200_LAYOUT_INTERLEAVED, "unknown velocity layout");
+    B200_REQUIRE(args_ok, args_msg);
+    B200_REQUIRE(tdiff != nullptr && T >= 1, "need at least one timestep");
+    B200_REQUIRE(m >= 1 && n >= 1 && (int64_t)m * n < ((int64_t)1 << 30), "grid must have 1 .. 2^30 pixels");
+    B200_REQUIRE(n_iter >= 0, "n_iter must be >= 0");
+    B200_REQUIRE(mode == B200_MODE_CONSTANT || mode == B200_MODE_NEAREST, "unsupported mode");
+    return 0;
+}
+
+// The fields of a trajectory launch that every driver sets alike, starting from `disp_prev` (or from rest).
+// T, the scales, the outputs, and the resume and batch fields are the driver's.
+SLParams sl_params(const double2 *Vi, const void *precip, const double *xy, const double *disp_prev, int m, int n,
+                   int row0, int rows, int n_iter, int mode, double outval, double vts, double td0) {
+    SLParams p;
+    memset(&p, 0, sizeof(p));
+    p.Vi = Vi;
+    p.precip = precip;
+    p.xy = xy;
+    p.m = m; p.n = n;
+    p.row0 = row0; p.rows = rows;
+    p.n_iter = n_iter;
+    p.mode = mode;
+    p.vts = vts;
+    p.td0 = td0;
+    p.cval = outval;
+    p.has_prev = disp_prev != nullptr;
+    p.init_mode = disp_prev ? SL_INIT_PREV : SL_INIT_FRESH;
+    p.disp_in = disp_prev;
+    return p;
+}
+
+// The trajectory kernel over T lead times, `per_launch` of them per launch; each launch after the first
+// resumes from the displacement and velocity increment the one before it left.  `out` (optional) holds
+// the T output planes.  `disp_steps` (optional) receives every launch's displacement, one (2,rows,n)
+// block per launch; without it the last launch's displacement goes to `disp_out` (optional).
+template <typename F, bool VF32>
+int sl_launches(const SLParams &start, const double *tdiff, int T, int per_launch, void *out, double *disp_out,
+                double *disp_steps, cudaStream_t stream) {
+    const size_t NB = (size_t)start.rows * start.n;
+    const int launches = (T + per_launch - 1) / per_launch;
+    b200::Scratch st_disp, st_vinc;
+    if (launches > 1) {
+        if (!disp_steps) B200_CUDA(st_disp.alloc(2 * NB * sizeof(double), stream));
         B200_CUDA(st_vinc.alloc(2 * NB * sizeof(double), stream));
     }
     dim3 block(SL_BX, SL_BY);
-    dim3 grid(b200::ceil_div(n, SL_BX), b200::ceil_div(rows, SL_BY));
-    for (int c = 0; c < nchunks; c++) {
-        SLParams p;
-        memset(&p, 0, sizeof(p));
-        p.Vi = vi_ptr;
-        p.precip = p_ptr;
-        p.xy = xy;
-        p.m = m; p.n = n;
-        p.row0 = row0; p.rows = rows;
-        p.n_iter = n_iter;
-        p.mode = mode;
-        p.vts = vts;
-        p.td0 = tdiff[0];
-        p.cval = outval;
-        p.has_prev = disp_prev != nullptr;
-        p.vel_f32 = sizeof(FV) == 4;
-        p.ti_offset = c * SL_MAX_T;
-        p.T = std::min(SL_MAX_T, T - p.ti_offset);
-        for (int i = 0; i < p.T; i++) p.scale[i] = tdiff[p.ti_offset + i] / vts;
-        if (c == 0) {
-            p.init_mode = disp_prev ? SL_INIT_PREV : SL_INIT_FRESH;
-            p.disp_in = disp_prev;
-        } else {
+    dim3 grid(b200::ceil_div(start.n, SL_BX), b200::ceil_div(start.rows, SL_BY));
+    const double *carried = nullptr;  // the displacement the previous launch wrote
+    for (int c = 0; c < launches; c++) {
+        SLParams p = start;
+        p.ti_offset = c * per_launch;
+        p.T = std::min(per_launch, T - p.ti_offset);
+        for (int i = 0; i < p.T; i++) p.scale[i] = tdiff[p.ti_offset + i] / p.vts;
+        if (c > 0) {
             p.init_mode = SL_INIT_RESUME;
-            p.disp_in = (const double *)st_disp.p;
+            p.disp_in = carried;
             p.vinc_in = (const double *)st_vinc.p;
         }
-        const bool last = (c == nchunks - 1);
-        p.disp_out = last ? disp_out : (double *)st_disp.p;
+        const bool last = (c == launches - 1);
+        p.disp_out = disp_steps ? disp_steps + (size_t)c * 2 * NB : last ? disp_out : (double *)st_disp.p;
         p.vinc_out = last ? nullptr : (double *)st_vinc.p;
-        p.out = precip ? (void *)((F *)out + (size_t)p.ti_offset * NB) : nullptr;
-        constexpr bool VF = sizeof(FV) == 4;
-        if (n_iter == 1)
-            sl_multistep_kernel<F, true, SL_BY, VF><<<grid, block, 0, stream>>>(p);
+        p.out = out ? (void *)((F *)out + (size_t)p.ti_offset * NB) : nullptr;
+        if (p.n_iter == 1)
+            sl_multistep_kernel<F, true, VF32><<<grid, block, 0, stream>>>(p);
         else
-            sl_multistep_kernel<F, false, SL_BY, VF><<<grid, block, 0, stream>>>(p);
+            sl_multistep_kernel<F, false, VF32><<<grid, block, 0, stream>>>(p);
         B200_LAUNCH_CHECK();
-    }
-    return 0;
-}
-
-// (2,m,n) planar or (m,n,2) interleaved velocity of dtype F -> (m,n) float2 (rounded to nearest)
-template <typename F>
-__global__ void __launch_bounds__(256)
-narrow_velocity_kernel(const F *__restrict__ V, float2 *__restrict__ Vf, size_t N, int interleaved) {
-    const size_t stride = (size_t)gridDim.x * blockDim.x;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += stride) {
-        float2 v;
-        if (interleaved) {
-            v.x = (float)__ldg(V + 2 * i);
-            v.y = (float)__ldg(V + 2 * i + 1);
-        } else {
-            v.x = (float)__ldg(V + i);
-            v.y = (float)__ldg(V + N + i);
-        }
-        Vf[i] = v;
-    }
-}
-
-// the float32-tap kernel with its exact fallback; restrictions checked by the caller
-template <typename FV, typename F>
-int sl_run_f32(const void *precip, const void *velocity, const double *disp_prev, const double *tdiff, int T,
-               double vts, double outval, int mode, int layout, int m, int n, int row0, int rows, void *out,
-               double *disp_out, unsigned long long *nfallback, cudaStream_t stream) {
-    const size_t N = (size_t)m * n;
-    b200::Scratch vi, vf;
-    const int sblocks = (int)std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 16);
-    const void *vi_ptr = velocity;  // exact float64 pairs, for the pixels that fall back
-    if (!(sizeof(FV) == 8 && layout == B200_LAYOUT_INTERLEAVED)) {
-        B200_CUDA(vi.alloc(N * sizeof(double2), stream));
-        vi_ptr = vi.p;
-        widen_velocity_kernel<FV><<<sblocks, 256, 0, stream>>>((const FV *)velocity, (double2 *)vi.p, N,
-                                                               layout == B200_LAYOUT_INTERLEAVED);
-        B200_LAUNCH_CHECK();
-    }
-    const void *vf_ptr = velocity;
-    if (!(sizeof(FV) == 4 && layout == B200_LAYOUT_INTERLEAVED)) {
-        B200_CUDA(vf.alloc(N * sizeof(float2), stream));
-        vf_ptr = vf.p;
-        narrow_velocity_kernel<FV><<<sblocks, 256, 0, stream>>>((const FV *)velocity, (float2 *)vf.p, N,
-                                                                layout == B200_LAYOUT_INTERLEAVED);
-        B200_LAUNCH_CHECK();
-    }
-    SLParams p;
-    memset(&p, 0, sizeof(p));
-    p.Vi = vi_ptr;
-    p.precip = precip;  // in its input type: sl_pixel<..., PT = F>
-    p.m = m; p.n = n;
-    p.row0 = row0; p.rows = rows;
-    p.n_iter = 1;
-    p.mode = mode;
-    p.vts = vts;
-    p.td0 = tdiff[0];
-    p.cval = outval;
-    p.has_prev = disp_prev != nullptr;
-    p.vel_f32 = sizeof(FV) == 4;
-    p.T = T;
-    SLFastParams q;
-    memset(&q, 0, sizeof(q));
-    for (int i = 0; i < T; i++) {
-        p.scale[i] = tdiff[i] / vts;
-        q.scale[i] = (float)p.scale[i];
-    }
-    q.s0 = (float)(tdiff[0] / vts);
-    q.Vf = (const float2 *)vf_ptr;
-    q.Pf = precip;
-    p.init_mode = disp_prev ? SL_INIT_PREV : SL_INIT_FRESH;
-    p.disp_in = disp_prev;
-    p.disp_out = disp_out;
-    p.out = out;
-    dim3 block(SL_BX, SL_BY);
-    dim3 grid(b200::ceil_div(n, SL_BX), b200::ceil_div(rows, SL_BY));
-    b200::Scratch lst;
-    const size_t NB = (size_t)rows * n;
-    B200_CUDA(lst.alloc(sizeof(int) * (NB + 4), stream));
-    q.nlist = (unsigned *)lst.p;
-    q.list = (int *)lst.p + 4;
-    B200_CUDA(cudaMemsetAsync(q.nlist, 0, sizeof(unsigned), stream));
-    sl_f32_kernel<F, sizeof(FV) == 4><<<grid, block, 0, stream>>>(p, q);
-    B200_LAUNCH_CHECK();
-    sl_f32_fixup_kernel<F, sizeof(FV) == 4><<<b200::num_sms() * 8, 128, 0, stream>>>(p, q.nlist, q.list, nfallback);
-    B200_LAUNCH_CHECK();
-    return 0;
-}
-
-// Displacement field after EVERY leadtime (for samplers other than the built-in order-1 warp):
-// the trajectory kernel run one leadtime per launch through the same resume mechanism that
-// chunks long sequences, so the arithmetic is that of the fused loop.
-template <typename FV>
-int sl_trajectories(const void *velocity, const double *xy, const double *disp_prev, const double *tdiff,
-                    int T, double vts, int n_iter, int layout, int m, int n, int row0, int rows,
-                    double *disp_steps, cudaStream_t stream) {
-    const size_t N = (size_t)m * n, NB = (size_t)rows * n;
-    b200::Scratch vi, st_vinc;
-    const int sblocks = (int)std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 16);
-    const void *vi_ptr = velocity;
-    if (!(sizeof(FV) == 8 && layout == B200_LAYOUT_INTERLEAVED)) {
-        B200_CUDA(vi.alloc(N * sizeof(double2), stream));
-        vi_ptr = vi.p;
-        widen_velocity_kernel<FV><<<sblocks, 256, 0, stream>>>(
-            (const FV *)velocity, (double2 *)vi.p, N, layout == B200_LAYOUT_INTERLEAVED);
-        B200_LAUNCH_CHECK();
-    }
-    B200_CUDA(st_vinc.alloc(2 * NB * sizeof(double), stream));
-    dim3 block(SL_BX, SL_BY);
-    dim3 grid(b200::ceil_div(n, SL_BX), b200::ceil_div(rows, SL_BY));
-    for (int c = 0; c < T; c++) {
-        SLParams p;
-        memset(&p, 0, sizeof(p));
-        p.Vi = vi_ptr;
-        p.xy = xy;
-        p.m = m; p.n = n;
-        p.row0 = row0; p.rows = rows;
-        p.n_iter = n_iter;
-        p.mode = B200_MODE_CONSTANT;
-        p.vts = vts;
-        p.td0 = tdiff[0];
-        p.has_prev = disp_prev != nullptr;
-        p.vel_f32 = sizeof(FV) == 4;
-        p.ti_offset = c;
-        p.T = 1;
-        p.scale[0] = tdiff[c] / vts;
-        if (c == 0) {
-            p.init_mode = disp_prev ? SL_INIT_PREV : SL_INIT_FRESH;
-            p.disp_in = disp_prev;
-        } else {
-            p.init_mode = SL_INIT_RESUME;
-            p.disp_in = disp_steps + (size_t)(c - 1) * 2 * NB;
-            p.vinc_in = (const double *)st_vinc.p;
-        }
-        p.disp_out = disp_steps + (size_t)c * 2 * NB;
-        p.vinc_out = (double *)st_vinc.p;
-        constexpr bool VF = sizeof(FV) == 4;
-        if (n_iter == 1)
-            sl_multistep_kernel<double, true, SL_BY, VF><<<grid, block, 0, stream>>>(p);
-        else
-            sl_multistep_kernel<double, false, SL_BY, VF><<<grid, block, 0, stream>>>(p);
-        B200_LAUNCH_CHECK();
+        carried = p.disp_out;
     }
     return 0;
 }
 
 }  // namespace
 
+// Displacement field after EVERY leadtime (for samplers other than the built-in order-1 warp):
+// the trajectory kernel run one leadtime per launch through the same resume mechanism that
+// chunks long sequences, so the arithmetic is that of the fused loop.
 extern "C" int b200_sl_trajectories(const void *velocity, const double *xy_coords, const double *disp_prev,
                                     const double *tdiff, int T, double vel_timestep, int n_iter,
                                     int velocity_dtype, int velocity_layout, int m, int n, int row_begin,
                                     int row_count, double *disp_steps, void *stream) {
-    B200_REQUIRE(row_begin >= 0 && row_count >= 1 && row_begin + row_count <= m, "row band out of range");
-    B200_REQUIRE(velocity_layout == B200_LAYOUT_PLANAR || velocity_layout == B200_LAYOUT_INTERLEAVED,
-                 "unknown velocity layout");
-    B200_REQUIRE(velocity != nullptr && disp_steps != nullptr, "velocity / disp_steps is NULL");
-    B200_REQUIRE(tdiff != nullptr && T >= 1, "need at least one timestep");
-    B200_REQUIRE(m >= 1 && n >= 1 && (int64_t)m * n < ((int64_t)1 << 30), "grid must have 1 .. 2^30 pixels");
-    B200_REQUIRE(n_iter >= 0, "n_iter must be >= 0");
+    if (int rc = check_band(m, n, row_begin, row_count, velocity_layout, velocity != nullptr && disp_steps != nullptr,
+                            "velocity / disp_steps is NULL", tdiff, T, n_iter, B200_MODE_CONSTANT))
+        return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    if (velocity_dtype == B200_F32)
-        return sl_trajectories<float>(velocity, xy_coords, disp_prev, tdiff, T, vel_timestep, n_iter,
-                                      velocity_layout, m, n, row_begin, row_count, disp_steps, s);
-    if (velocity_dtype == B200_F64)
-        return sl_trajectories<double>(velocity, xy_coords, disp_prev, tdiff, T, vel_timestep, n_iter,
-                                       velocity_layout, m, n, row_begin, row_count, disp_steps, s);
-    b200::set_error("unknown velocity dtype %d", velocity_dtype);
-    return B200_EINVAL;
+    return with_dtype(velocity_dtype, [&](auto fv) {
+        using FV = typename decltype(fv)::type;
+        b200::Scratch vi;
+        const double2 *Vi;
+        if (int rc = velocity_pairs<double2, FV>(velocity, velocity_layout, (size_t)m * n, vi, Vi, s)) return rc;
+        const SLParams p = sl_params(Vi, nullptr, xy_coords, disp_prev, m, n, row_begin, row_count, n_iter,
+                                     B200_MODE_CONSTANT, 0.0, vel_timestep, tdiff[0]);
+        return sl_launches<double, sizeof(FV) == 4>(p, tdiff, T, 1, nullptr, nullptr, disp_steps, s);
+    });
 }
 
 extern "C" int b200_sl_extrapolate_rows(const void *precip, const void *velocity,
@@ -760,27 +661,31 @@ extern "C" int b200_sl_extrapolate_rows(const void *precip, const void *velocity
                                         double outval, int mode, int velocity_dtype, int velocity_layout,
                                         int precip_dtype, int m, int n, int row_begin, int row_count,
                                         void *out, double *disp_out, void *stream) {
-    B200_REQUIRE(row_begin >= 0 && row_count >= 1 && row_begin + row_count <= m, "row band out of range");
-    B200_REQUIRE(velocity_layout == B200_LAYOUT_PLANAR || velocity_layout == B200_LAYOUT_INTERLEAVED,
-                 "unknown velocity layout");
-    B200_REQUIRE(velocity != nullptr, "velocity is NULL");
-    B200_REQUIRE(tdiff != nullptr && T >= 1, "need at least one timestep");
-    B200_REQUIRE(m >= 1 && n >= 1 && (int64_t)m * n < ((int64_t)1 << 30), "grid must have 1 .. 2^30 pixels");
-    B200_REQUIRE(n_iter >= 0, "n_iter must be >= 0");
-    B200_REQUIRE(mode == B200_MODE_CONSTANT || mode == B200_MODE_NEAREST, "unsupported mode");
+    if (int rc = check_band(m, n, row_begin, row_count, velocity_layout, velocity != nullptr, "velocity is NULL",
+                            tdiff, T, n_iter, mode))
+        return rc;
     B200_REQUIRE((precip == nullptr) == (out == nullptr), "precip and out must both be given or both NULL");
     B200_REQUIRE(precip != nullptr || disp_out != nullptr, "nothing to compute");
     cudaStream_t s = (cudaStream_t)stream;
-#define SL_DISPATCH(FV, FP)                                                                  \
-    return sl_run<FV, FP>(precip, velocity, xy_coords, disp_prev, tdiff, T, vel_timestep, n_iter, \
-                          outval, mode, velocity_layout, m, n, row_begin, row_count, out, disp_out, s)
-    if (velocity_dtype == B200_F32 && precip_dtype == B200_F32) SL_DISPATCH(float, float);
-    if (velocity_dtype == B200_F32 && precip_dtype == B200_F64) SL_DISPATCH(float, double);
-    if (velocity_dtype == B200_F64 && precip_dtype == B200_F32) SL_DISPATCH(double, float);
-    if (velocity_dtype == B200_F64 && precip_dtype == B200_F64) SL_DISPATCH(double, double);
-#undef SL_DISPATCH
-    b200::set_error("unknown field dtypes %d / %d", velocity_dtype, precip_dtype);
-    return B200_EINVAL;
+    return with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
+        using FV = typename decltype(fv)::type;
+        using F = typename decltype(fp)::type;
+        const size_t N = (size_t)m * n;  // full frame (inputs)
+        b200::Scratch vi, pw;
+        // widen the fields to float64 once (exact), so the trajectory loop issues no conversions
+        const double2 *Vi;
+        if (int rc = velocity_pairs<double2, FV>(velocity, velocity_layout, N, vi, Vi, s)) return rc;
+        const void *p_ptr = precip;
+        if (precip && sizeof(F) == 4) {
+            B200_CUDA(pw.alloc(N * sizeof(double), s));
+            p_ptr = pw.p;
+            widen_field_kernel<<<stream_blocks(N, 16), 256, 0, s>>>((const float *)precip, (double *)pw.p, N);
+            B200_LAUNCH_CHECK();
+        }
+        const SLParams p = sl_params(Vi, p_ptr, xy_coords, disp_prev, m, n, row_begin, row_count, n_iter, mode,
+                                     outval, vel_timestep, tdiff[0]);
+        return sl_launches<F, sizeof(FV) == 4>(p, tdiff, T, SL_MAX_T, out, disp_out, nullptr, s);
+    });
 }
 
 // Opt-in float32-tap variant of b200_sl_extrapolate_rows (see sl_f32_kernel): n_iter = 1, pixel-grid
@@ -792,28 +697,52 @@ extern "C" int b200_sl_extrapolate_rows_f32(const void *precip, const void *velo
                                             int mode, int velocity_dtype, int velocity_layout, int precip_dtype,
                                             int m, int n, int row_begin, int row_count, void *out,
                                             double *disp_out, unsigned long long *fallback_count, void *stream) {
-    B200_REQUIRE(row_begin >= 0 && row_count >= 1 && row_begin + row_count <= m, "row band out of range");
-    B200_REQUIRE(velocity_layout == B200_LAYOUT_PLANAR || velocity_layout == B200_LAYOUT_INTERLEAVED,
-                 "unknown velocity layout");
-    B200_REQUIRE(velocity != nullptr && precip != nullptr && out != nullptr, "precip, velocity and out are required");
-    B200_REQUIRE(tdiff != nullptr && T >= 1, "need at least one timestep");
-    B200_REQUIRE(m >= 1 && n >= 1 && (int64_t)m * n < ((int64_t)1 << 30), "grid must have 1 .. 2^30 pixels");
-    B200_REQUIRE(mode == B200_MODE_CONSTANT || mode == B200_MODE_NEAREST, "unsupported mode");
+    if (int rc = check_band(m, n, row_begin, row_count, velocity_layout,
+                            velocity != nullptr && precip != nullptr && out != nullptr,
+                            "precip, velocity and out are required", tdiff, T, 1, mode))
+        return rc;
     if (T > SL_MAX_T) {
         b200::set_error("the float32-tap kernel takes at most %d timesteps per call", SL_MAX_T);
         return B200_ENOTSUP;
     }
     cudaStream_t s = (cudaStream_t)stream;
-#define SL_DISPATCH(FV, FP)                                                                            \
-    return sl_run_f32<FV, FP>(precip, velocity, disp_prev, tdiff, T, vel_timestep, outval, mode, velocity_layout, \
-                              m, n, row_begin, row_count, out, disp_out, fallback_count, s)
-    if (velocity_dtype == B200_F32 && precip_dtype == B200_F32) SL_DISPATCH(float, float);
-    if (velocity_dtype == B200_F32 && precip_dtype == B200_F64) SL_DISPATCH(float, double);
-    if (velocity_dtype == B200_F64 && precip_dtype == B200_F32) SL_DISPATCH(double, float);
-    if (velocity_dtype == B200_F64 && precip_dtype == B200_F64) SL_DISPATCH(double, double);
-#undef SL_DISPATCH
-    b200::set_error("unknown field dtypes %d / %d", velocity_dtype, precip_dtype);
-    return B200_EINVAL;
+    return with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
+        using FV = typename decltype(fv)::type;
+        using F = typename decltype(fp)::type;
+        constexpr bool VF32 = sizeof(FV) == 4;
+        const size_t N = (size_t)m * n, NB = (size_t)row_count * n;
+        b200::Scratch vi, vf, lst;
+        const double2 *Vi;  // exact float64 pairs, for the pixels that fall back
+        if (int rc = velocity_pairs<double2, FV>(velocity, velocity_layout, N, vi, Vi, s)) return rc;
+        const float2 *Vf;
+        if (int rc = velocity_pairs<float2, FV>(velocity, velocity_layout, N, vf, Vf, s)) return rc;
+        // the precipitation in its input type: sl_pixel<..., PT = F>
+        SLParams p = sl_params(Vi, precip, nullptr, disp_prev, m, n, row_begin, row_count, 1, mode, outval,
+                               vel_timestep, tdiff[0]);
+        p.T = T;
+        p.disp_out = disp_out;
+        p.out = out;
+        SLFastParams q;
+        memset(&q, 0, sizeof(q));
+        for (int i = 0; i < T; i++) {
+            p.scale[i] = tdiff[i] / vel_timestep;
+            q.scale[i] = (float)p.scale[i];
+        }
+        q.s0 = (float)(tdiff[0] / vel_timestep);
+        q.Vf = Vf;
+        q.Pf = precip;
+        B200_CUDA(lst.alloc(sizeof(int) * (NB + 4), s));
+        q.nlist = (unsigned *)lst.p;
+        q.list = (int *)lst.p + 4;
+        B200_CUDA(cudaMemsetAsync(q.nlist, 0, sizeof(unsigned), s));
+        dim3 block(SL_BX, SL_BY);
+        dim3 grid(b200::ceil_div(n, SL_BX), b200::ceil_div(row_count, SL_BY));
+        sl_f32_kernel<F, VF32><<<grid, block, 0, s>>>(p, q);
+        B200_LAUNCH_CHECK();
+        sl_f32_fixup_kernel<F, VF32><<<b200::num_sms() * 8, 128, 0, s>>>(p, q.nlist, q.list, fallback_count);
+        B200_LAUNCH_CHECK();
+        return 0;
+    });
 }
 
 extern "C" int b200_sl_extrapolate(const void *precip, const void *velocity,
@@ -875,25 +804,46 @@ extern "C" int b200_sl_interleave_velocity(const void *velocity, int velocity_dt
                                            void *out, void *stream) {
     B200_REQUIRE(velocity != nullptr && out != nullptr && m >= 1 && n >= 1, "bad arguments");
     const size_t N = (size_t)m * n;
-    const int blocks = (int)std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 16);
     cudaStream_t s = (cudaStream_t)stream;
-    if (velocity_dtype == B200_F32)
-        interleave_kernel<float, float2><<<blocks, 256, 0, s>>>((const float *)velocity, (float2 *)out, N);
-    else if (velocity_dtype == B200_F64)
-        interleave_kernel<double, double2><<<blocks, 256, 0, s>>>((const double *)velocity, (double2 *)out, N);
-    else {
-        b200::set_error("unknown velocity dtype %d", velocity_dtype);
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
-    return 0;
+    return with_dtype(velocity_dtype, [&](auto fv) {
+        using F = typename decltype(fv)::type;
+        using F2 = std::conditional_t<sizeof(F) == 4, float2, double2>;
+        relayout_kernel<F, F2, false><<<stream_blocks(N, 16), 256, 0, s>>>((const F *)velocity, (F2 *)out, N);
+        B200_LAUNCH_CHECK();
+        return 0;
+    });
 }
 
-// BPS motion perturbation (pysteps/noise/motion.py:129-180) applied at the grid nodes while the
-// field is re-laid out for the trajectory kernel: out = V + (a*V_par + b*V_perp)/vsf with
-// V_par = V/|V| (zero where |V| <= 1e-12), V_perp = (-V_par.y, V_par.x), a = g_par(t)*eps_par,
-// b = g_perp(t)*eps_perp.  The norm and the division run in the field's own dtype, as NumPy does
+// BPS motion perturbation (pysteps/noise/motion.py:129-180) at one grid node: out = V + (a*V_par + b*V_perp)/vsf
+// with V_par = V/|V| (zero where |V| <= 1e-12), V_perp = (-V_par.y, V_par.x), a = g_par(t)*eps_par,
+// b = g_perp(t)*eps_perp; WHAT selects V_par alone (B200_BPS_UNIT) or the perturbation alone
+// (B200_BPS_PERTURBATION).  The norm and the division run in the field's own dtype, as NumPy does
 // (linalg.norm and V/N keep float32; the result is stored into a float64 array, :138-139).
+template <typename F, int WHAT>
+static __device__ __forceinline__ double2 bps_point(const F vx, const F vy, double a, double b, double vsf) {
+    double nx, ny;
+    if (sizeof(F) == 4) {
+        const float nrm = __fsqrt_rn(__fadd_rn(__fmul_rn((float)vx, (float)vx), __fmul_rn((float)vy, (float)vy)));
+        const bool ok = nrm > (float)1e-12;  // NaN compares false
+        nx = ok ? (double)__fdiv_rn((float)vx, nrm) : 0.0;
+        ny = ok ? (double)__fdiv_rn((float)vy, nrm) : 0.0;
+    } else {
+        const double nrm = __dsqrt_rn(__dadd_rn(__dmul_rn((double)vx, (double)vx), __dmul_rn((double)vy, (double)vy)));
+        const bool ok = nrm > 1e-12;
+        nx = ok ? __ddiv_rn((double)vx, nrm) : 0.0;
+        ny = ok ? __ddiv_rn((double)vy, nrm) : 0.0;
+    }
+    if (WHAT == B200_BPS_UNIT) return make_double2(nx, ny);
+    double ox = __ddiv_rn(__dadd_rn(__dmul_rn(a, nx), __dmul_rn(b, -ny)), vsf);
+    double oy = __ddiv_rn(__dadd_rn(__dmul_rn(a, ny), __dmul_rn(b, nx)), vsf);
+    if (WHAT != B200_BPS_PERTURBATION) {
+        ox = __dadd_rn((double)vx, ox);
+        oy = __dadd_rn((double)vy, oy);
+    }
+    return make_double2(ox, oy);
+}
+
+// the perturbation applied while the field is re-laid out for the trajectory kernel
 template <typename F, int WHAT>
 __global__ void __launch_bounds__(256)
 bps_perturb_kernel(const F *__restrict__ V, double *__restrict__ out, size_t N, double a, double b,
@@ -902,37 +852,14 @@ bps_perturb_kernel(const F *__restrict__ V, double *__restrict__ out, size_t N, 
     int bad = 0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += stride) {
         const F vx = __ldg(V + i), vy = __ldg(V + N + i);
-        double nx, ny;
-        if (sizeof(F) == 4) {
-            const float nrm = __fsqrt_rn(__fadd_rn(__fmul_rn((float)vx, (float)vx), __fmul_rn((float)vy, (float)vy)));
-            const bool ok = nrm > (float)1e-12;  // NaN compares false
-            nx = ok ? (double)__fdiv_rn((float)vx, nrm) : 0.0;
-            ny = ok ? (double)__fdiv_rn((float)vy, nrm) : 0.0;
-        } else {
-            const double nrm = __dsqrt_rn(__dadd_rn(__dmul_rn((double)vx, (double)vx), __dmul_rn((double)vy, (double)vy)));
-            const bool ok = nrm > 1e-12;
-            nx = ok ? __ddiv_rn((double)vx, nrm) : 0.0;
-            ny = ok ? __ddiv_rn((double)vy, nrm) : 0.0;
-        }
-        double ox, oy;
-        if (WHAT == B200_BPS_UNIT) {
-            ox = nx;
-            oy = ny;
-        } else {
-            ox = __ddiv_rn(__dadd_rn(__dmul_rn(a, nx), __dmul_rn(b, -ny)), vsf);
-            oy = __ddiv_rn(__dadd_rn(__dmul_rn(a, ny), __dmul_rn(b, nx)), vsf);
-            if (WHAT != B200_BPS_PERTURBATION) {
-                ox = __dadd_rn((double)vx, ox);
-                oy = __dadd_rn((double)vy, oy);
-            }
-        }
-        bad += !isfinite(ox);
-        bad += !isfinite(oy);
+        const double2 o = bps_point<F, WHAT>(vx, vy, a, b, vsf);
+        bad += !isfinite(o.x);
+        bad += !isfinite(o.y);
         if (WHAT == B200_BPS_FIELD_INTERLEAVED) {
-            reinterpret_cast<double2 *>(out)[i] = make_double2(ox, oy);
+            reinterpret_cast<double2 *>(out)[i] = o;
         } else {
-            out[i] = ox;
-            out[N + i] = oy;
+            out[i] = o.x;
+            out[N + i] = o.y;
         }
     }
     // number of non-finite output elements (the check of semilagrangian.py:116-123 on the
@@ -946,7 +873,7 @@ template <typename F>
 static int bps_launch(const void *velocity, size_t N, double a, double b, double vsf, int what, double *out,
                       double *nnf, cudaStream_t s) {
     if (nnf) B200_CUDA(cudaMemsetAsync(nnf, 0, sizeof(double), s));
-    const int blocks = (int)std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 16);
+    const int blocks = stream_blocks(N, 16);
     const F *V = (const F *)velocity;
     switch (what) {
     case B200_BPS_FIELD_INTERLEAVED:
@@ -986,83 +913,14 @@ bps_perturb_batched_kernel(const F *__restrict__ V, double2 *__restrict__ out, s
     int bad = 0;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += stride) {
         const F vx = __ldg(V + i), vy = __ldg(V + N + i);
-        double nx, ny;  // unit vector in the field's own dtype (bps_perturb_kernel)
-        if (sizeof(F) == 4) {
-            const float nrm = __fsqrt_rn(__fadd_rn(__fmul_rn((float)vx, (float)vx), __fmul_rn((float)vy, (float)vy)));
-            const bool ok = nrm > (float)1e-12;
-            nx = ok ? (double)__fdiv_rn((float)vx, nrm) : 0.0;
-            ny = ok ? (double)__fdiv_rn((float)vy, nrm) : 0.0;
-        } else {
-            const double nrm = __dsqrt_rn(__dadd_rn(__dmul_rn((double)vx, (double)vx), __dmul_rn((double)vy, (double)vy)));
-            const bool ok = nrm > 1e-12;
-            nx = ok ? __ddiv_rn((double)vx, nrm) : 0.0;
-            ny = ok ? __ddiv_rn((double)vy, nrm) : 0.0;
-        }
-        const double ox = __dadd_rn((double)vx, __ddiv_rn(__dadd_rn(__dmul_rn(a, nx), __dmul_rn(b, -ny)), vsf));
-        const double oy = __dadd_rn((double)vy, __ddiv_rn(__dadd_rn(__dmul_rn(a, ny), __dmul_rn(b, nx)), vsf));
-        bad += !isfinite(ox);
-        bad += !isfinite(oy);
-        o[i] = make_double2(ox, oy);
+        const double2 v = bps_point<F, B200_BPS_FIELD_INTERLEAVED>(vx, vy, a, b, vsf);
+        bad += !isfinite(v.x);
+        bad += !isfinite(v.y);
+        o[i] = v;
     }
     if (n_nonfinite != nullptr && __any_sync(0xffffffffu, bad != 0)) {
         if (bad) atomicAdd(n_nonfinite + mem, (double)bad);
     }
-}
-
-template <typename FV, typename F>
-static int sl_step_batched(const void *velocity, int m, int n, int members, const double *coefs, double vsf,
-                           const void *precip, const double *disp_prev, double tdiff, double vts, double outval,
-                           int mode, void *out, double *disp_out, double *n_nonfinite, cudaStream_t stream) {
-    const size_t N = (size_t)m * n;
-    const int ch_max = std::min(members, SL_BATCH);
-    b200::Scratch vp, pw;
-    B200_CUDA(vp.alloc((size_t)ch_max * N * sizeof(double2), stream));
-    if (sizeof(F) == 4) B200_CUDA(pw.alloc((size_t)ch_max * N * sizeof(double), stream));
-    if (n_nonfinite) B200_CUDA(cudaMemsetAsync(n_nonfinite, 0, sizeof(double) * members, stream));
-    const int sblocks = (int)std::min<size_t>((N + 255) / 256, (size_t)b200::num_sms() * 8);
-    for (int m0 = 0; m0 < members; m0 += SL_BATCH) {
-        const int ch = std::min(SL_BATCH, members - m0);
-        BpsBatch ab;
-        for (int j = 0; j < SL_BATCH; j++) {
-            ab.a[j] = j < ch ? coefs[2 * (m0 + j)] : 0.0;
-            ab.b[j] = j < ch ? coefs[2 * (m0 + j) + 1] : 0.0;
-        }
-        bps_perturb_batched_kernel<FV><<<dim3(sblocks, ch), 256, 0, stream>>>(
-            (const FV *)velocity, (double2 *)vp.p, N, ab, vsf, n_nonfinite ? n_nonfinite + m0 : nullptr);
-        B200_LAUNCH_CHECK();
-        const void *p_ptr = (const F *)precip + (size_t)m0 * N;
-        if (sizeof(F) == 4) {
-            const int wblocks = (int)std::min<size_t>(((size_t)ch * N + 255) / 256, (size_t)b200::num_sms() * 16);
-            widen_field_kernel<<<wblocks, 256, 0, stream>>>((const float *)p_ptr, (double *)pw.p, (size_t)ch * N);
-            B200_LAUNCH_CHECK();
-            p_ptr = pw.p;
-        }
-        SLParams p;
-        memset(&p, 0, sizeof(p));
-        p.Vi = vp.p;
-        p.precip = p_ptr;
-        p.m = m; p.n = n;
-        p.row0 = 0; p.rows = m;
-        p.n_iter = 1;
-        p.mode = mode;
-        p.vts = vts;
-        p.td0 = tdiff;
-        p.cval = outval;
-        p.has_prev = disp_prev != nullptr;
-        p.vel_f32 = 0;  // the perturbed field is float64 (noise/motion.py:138-139)
-        p.T = 1;
-        p.scale[0] = tdiff / vts;
-        p.init_mode = disp_prev ? SL_INIT_PREV : SL_INIT_FRESH;
-        p.disp_in = disp_prev ? disp_prev + (size_t)m0 * 2 * N : nullptr;
-        p.disp_out = disp_out + (size_t)m0 * 2 * N;
-        p.out = (F *)out + (size_t)m0 * N;
-        p.zs_vi = N; p.zs_precip = N; p.zs_disp = 2 * N; p.zs_out = N;
-        dim3 block(SL_BX, SL_BY);
-        dim3 grid(b200::ceil_div(n, SL_BX), b200::ceil_div(m, SL_BY), ch);
-        sl_multistep_kernel<F, true, SL_BY, false, true><<<grid, block, 0, stream>>>(p);
-        B200_LAUNCH_CHECK();
-    }
-    return 0;
 }
 
 extern "C" int b200_sl_step_batched(const void *velocity, int velocity_dtype, int m, int n, int members,
@@ -1073,16 +931,49 @@ extern "C" int b200_sl_step_batched(const void *velocity, int velocity_dtype, in
     B200_REQUIRE(m >= 1 && n >= 1 && (int64_t)m * n < ((int64_t)1 << 30) && members >= 1, "bad sizes");
     B200_REQUIRE(mode == B200_MODE_CONSTANT || mode == B200_MODE_NEAREST, "unsupported mode");
     cudaStream_t s = (cudaStream_t)stream;
-#define SLB(FV, FP)                                                                                         \
-    return sl_step_batched<FV, FP>(velocity, m, n, members, pert_coefs, vsf, precip, disp_prev, tdiff,      \
-                                   vel_timestep, outval, mode, out, disp_out, n_nonfinite, s)
-    if (velocity_dtype == B200_F32 && precip_dtype == B200_F32) SLB(float, float);
-    if (velocity_dtype == B200_F32 && precip_dtype == B200_F64) SLB(float, double);
-    if (velocity_dtype == B200_F64 && precip_dtype == B200_F32) SLB(double, float);
-    if (velocity_dtype == B200_F64 && precip_dtype == B200_F64) SLB(double, double);
-#undef SLB
-    b200::set_error("unknown field dtypes %d / %d", velocity_dtype, precip_dtype);
-    return B200_EINVAL;
+    return with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
+        using FV = typename decltype(fv)::type;
+        using F = typename decltype(fp)::type;
+        const size_t N = (size_t)m * n;
+        const int ch_max = std::min(members, SL_BATCH);
+        b200::Scratch vp, pw;
+        B200_CUDA(vp.alloc((size_t)ch_max * N * sizeof(double2), s));
+        if (sizeof(F) == 4) B200_CUDA(pw.alloc((size_t)ch_max * N * sizeof(double), s));
+        if (n_nonfinite) B200_CUDA(cudaMemsetAsync(n_nonfinite, 0, sizeof(double) * members, s));
+        const int sblocks = stream_blocks(N, 8);
+        for (int m0 = 0; m0 < members; m0 += SL_BATCH) {
+            const int ch = std::min(SL_BATCH, members - m0);
+            BpsBatch ab;
+            for (int j = 0; j < SL_BATCH; j++) {
+                ab.a[j] = j < ch ? pert_coefs[2 * (m0 + j)] : 0.0;
+                ab.b[j] = j < ch ? pert_coefs[2 * (m0 + j) + 1] : 0.0;
+            }
+            bps_perturb_batched_kernel<FV><<<dim3(sblocks, ch), 256, 0, s>>>(
+                (const FV *)velocity, (double2 *)vp.p, N, ab, vsf, n_nonfinite ? n_nonfinite + m0 : nullptr);
+            B200_LAUNCH_CHECK();
+            const void *p_ptr = (const F *)precip + (size_t)m0 * N;
+            if (sizeof(F) == 4) {
+                widen_field_kernel<<<stream_blocks((size_t)ch * N, 16), 256, 0, s>>>((const float *)p_ptr,
+                                                                                     (double *)pw.p, (size_t)ch * N);
+                B200_LAUNCH_CHECK();
+                p_ptr = pw.p;
+            }
+            const double *d_prev = disp_prev ? disp_prev + (size_t)m0 * 2 * N : nullptr;
+            SLParams p = sl_params((const double2 *)vp.p, p_ptr, nullptr, d_prev, m, n, 0, m, 1, mode, outval,
+                                   vel_timestep, tdiff);
+            p.T = 1;
+            p.scale[0] = tdiff / vel_timestep;
+            p.disp_out = disp_out + (size_t)m0 * 2 * N;
+            p.out = (F *)out + (size_t)m0 * N;
+            p.zs_vi = N; p.zs_precip = N; p.zs_disp = 2 * N; p.zs_out = N;
+            dim3 block(SL_BX, SL_BY);
+            dim3 grid(b200::ceil_div(n, SL_BX), b200::ceil_div(m, SL_BY), ch);
+            // VF32 = false: the perturbed field is float64 (noise/motion.py:138-139)
+            sl_multistep_kernel<F, true, false, true><<<grid, block, 0, s>>>(p);
+            B200_LAUNCH_CHECK();
+        }
+        return 0;
+    });
 }
 
 extern "C" int b200_bps_perturb_velocity(const void *velocity, int velocity_dtype, int m, int n,
@@ -1091,8 +982,7 @@ extern "C" int b200_bps_perturb_velocity(const void *velocity, int velocity_dtyp
     B200_REQUIRE(velocity != nullptr && out != nullptr && m >= 1 && n >= 1, "bad arguments");
     const size_t N = (size_t)m * n;
     cudaStream_t s = (cudaStream_t)stream;
-    if (velocity_dtype == B200_F32) return bps_launch<float>(velocity, N, a_par, a_perp, vsf, what, out, n_nonfinite, s);
-    if (velocity_dtype == B200_F64) return bps_launch<double>(velocity, N, a_par, a_perp, vsf, what, out, n_nonfinite, s);
-    b200::set_error("unknown velocity dtype %d", velocity_dtype);
-    return B200_EINVAL;
+    return with_dtype(velocity_dtype, [&](auto fv) {
+        return bps_launch<typename decltype(fv)::type>(velocity, N, a_par, a_perp, vsf, what, out, n_nonfinite, s);
+    });
 }

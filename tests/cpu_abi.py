@@ -9,6 +9,7 @@ host logic with the live reference on thousands of argument combinations.
 """
 import contextlib
 import ctypes
+import threading
 from unittest import mock
 
 import numpy as np
@@ -543,6 +544,15 @@ def emulated():
         st.enter_context(mock.patch.object(torch.cuda, "stream", lambda s: contextlib.nullcontext()))
         st.enter_context(mock.patch.object(torch.cuda, "current_device", lambda: 0))
         _side.clear()
+        # The LK module caches side streams, pixel grids and pinned buffers per device and thread.  Emulated
+        # calls get empty caches and leave the real ones as they were: a real stream cached by an earlier
+        # device run rejects the stand-in events, and a host tensor cached here would reach a later
+        # device run as a device pointer.
+        from pysteps_b200.motion import lucaskanade
+        st.enter_context(mock.patch.dict(lucaskanade._side_streams, clear=True))
+        st.enter_context(mock.patch.dict(lucaskanade._grids, clear=True))
+        st.enter_context(mock.patch.object(lucaskanade, "_readback", threading.local()))
+        st.enter_context(mock.patch.object(lucaskanade, "_plan_pin", threading.local()))
         st.enter_context(mock.patch.object(torch.cuda, "current_stream", lambda *a: _Stream()))
         # a device tensor's .cpu() is a fresh host copy; keep that property for the stand-ins
         st.enter_context(mock.patch.object(torch.Tensor, "cpu", lambda self, *a, **k: self.clone()))

@@ -68,3 +68,66 @@ def test_get_method_contract():
     assert out.shape == (3, 10, 10) and np.array_equal(out[2], precip)
     out, disp = eulerian_persistence(precip, None, [1, 2], return_displacement=True)
     assert out.shape == (2, 10, 10) and not disp.any()
+
+
+def test_sl_entry_points_name_the_first_broken_rule():
+    """The semi-Lagrangian entry points check their arguments in a fixed order and report the first
+    rule an input breaks, with its error code; unknown dtype codes are named in the message.  Every
+    call here is refused before any device work, so no GPU is needed."""
+    lib = _lib.load()
+    td = np.ones(40)
+    tdp = td.ctypes.data_as(_lib.c_dp)
+    buf = 0x1000  # a device pointer that is never dereferenced: each call below is refused first
+    einval, enotsup = 100001, 100002
+
+    def check(fn, defaults, want_rc, want_msg, **kw):
+        args = dict(defaults, **kw)
+        rc = getattr(lib, fn)(*args.values())
+        msg = lib.b200_last_error().decode().split(" (")[0]
+        assert (rc, msg) == (want_rc, want_msg), (fn, kw)
+
+    rows = dict(precip=buf, velocity=buf, xy=None, disp_prev=None, tdiff=tdp, T=4, vts=1.0, n_iter=1, outval=0.0,
+                mode=0, vdt=1, layout=0, pdt=1, m=8, n=8, r0=0, rows=8, out=buf, disp_out=None, stream=None)
+    f32 = dict(precip=buf, velocity=buf, disp_prev=None, tdiff=tdp, T=4, vts=1.0, outval=0.0, mode=0, vdt=1,
+               layout=0, pdt=1, m=8, n=8, r0=0, rows=8, out=buf, disp_out=None, fallback=None, stream=None)
+    traj = dict(velocity=buf, xy=None, disp_prev=None, tdiff=tdp, T=4, vts=1.0, n_iter=1, vdt=1, layout=0, m=8,
+                n=8, r0=0, rows=8, steps=buf, stream=None)
+    for fn, d in (("b200_sl_extrapolate_rows", rows), ("b200_sl_extrapolate_rows_f32", f32),
+                  ("b200_sl_trajectories", traj)):
+        null = {"b200_sl_extrapolate_rows": "velocity is NULL",
+                "b200_sl_extrapolate_rows_f32": "precip, velocity and out are required",
+                "b200_sl_trajectories": "velocity / disp_steps is NULL"}[fn]
+        check(fn, d, einval, "row band out of range", r0=-1, layout=5, velocity=None)
+        check(fn, d, einval, "row band out of range", r0=4, rows=5)
+        check(fn, d, einval, "row band out of range", rows=0)
+        check(fn, d, einval, "unknown velocity layout", layout=2, velocity=None)
+        check(fn, d, einval, null, velocity=None, tdiff=None)
+        check(fn, d, einval, "need at least one timestep", tdiff=None, m=8, n=0)
+        check(fn, d, einval, "need at least one timestep", T=0)
+        check(fn, d, einval, "grid must have 1 .. 2^30 pixels", n=0)
+        check(fn, d, einval, "grid must have 1 .. 2^30 pixels", n=1 << 27)
+    check("b200_sl_extrapolate_rows_f32", f32, einval, "precip, velocity and out are required", precip=None)
+    check("b200_sl_extrapolate_rows_f32", f32, einval, "precip, velocity and out are required", out=None)
+    check("b200_sl_trajectories", traj, einval, "velocity / disp_steps is NULL", steps=None)
+    for fn, d in (("b200_sl_extrapolate_rows", rows), ("b200_sl_trajectories", traj)):
+        check(fn, d, einval, "n_iter must be >= 0", n_iter=-1, **({"mode": 7} if "mode" in d else {}))
+    for fn, d in (("b200_sl_extrapolate_rows", rows), ("b200_sl_extrapolate_rows_f32", f32)):
+        check(fn, d, einval, "unsupported mode", mode=7, T=33)
+        check(fn, d, einval, "unknown field dtypes 7 / 1", vdt=7)
+        check(fn, d, einval, "unknown field dtypes 1 / -1", pdt=-1)
+    check("b200_sl_extrapolate_rows", rows, einval, "precip and out must both be given or both NULL", out=None)
+    check("b200_sl_extrapolate_rows", rows, einval, "precip and out must both be given or both NULL", precip=None)
+    check("b200_sl_extrapolate_rows", rows, einval, "nothing to compute", precip=None, out=None)
+    check("b200_sl_extrapolate_rows", rows, einval, "unknown field dtypes 2 / 1", precip=None, out=None,
+          disp_out=buf, vdt=2)
+    check("b200_sl_extrapolate_rows_f32", f32, enotsup, "the float32-tap kernel takes at most 32 timesteps per call",
+          T=33, vdt=7)
+    check("b200_sl_trajectories", traj, einval, "unknown velocity dtype 4", vdt=4)
+
+    batched = dict(velocity=buf, vdt=1, m=8, n=8, members=3, coefs=buf, vsf=1.0, precip=buf, pdt=1, disp_prev=None,
+                   tdiff=1.0, vts=1.0, outval=0.0, mode=0, out=buf, disp_out=buf, nnf=None, stream=None)
+    check("b200_sl_step_batched", batched, einval, "unknown field dtypes 0 / 5", vdt=0, pdt=5)
+    check("b200_sl_interleave_velocity", dict(velocity=buf, vdt=3, m=8, n=8, out=buf, stream=None), einval,
+          "unknown velocity dtype 3")
+    bps = dict(velocity=buf, vdt=3, m=8, n=8, a=0.0, b=0.0, vsf=1.0, what=0, out=buf, nnf=None, stream=None)
+    check("b200_bps_perturb_velocity", bps, einval, "unknown velocity dtype 3")

@@ -9,7 +9,7 @@ prints the table:
     kernel, mean per step: what b200_idw_fill (or the plan + planned fill) costs, kernel by kernel
   - the idle time on the main stream between the end of decluster_kernel and the start of the first fill
     kernel (idw32_kernel / idw_kernel / idw_plan_const_kernel): the gap the GPU waits for the host
-  - the re-layout of the field before the trajectory kernel (interleave_kernel / widen_velocity_kernel)
+  - the re-layout of the field before the trajectory kernel (relayout_kernel)
 The L2 is flushed between steps as in bench.py (outside the steps).
 """
 import argparse
@@ -24,7 +24,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 FILL_FIRST = ("idw32_kernel", "idw_kernel", "idw_plan_const_kernel")
-RELAYOUT = ("interleave_kernel", "widen_velocity_kernel")
+RELAYOUT = ("relayout_kernel",)
 
 
 def _short(name):
@@ -33,7 +33,7 @@ def _short(name):
     base = name.replace("(anonymous namespace)::", "").split("(")[0]
     for tok in ("idw32_kernel", "idw_kernel", "idw_plan_const_kernel", "idw_plan_kernel", "kd_build_kernel",
                 "kd_build_serial_kernel", "idw_fix_warp_kernel", "idw_fix_kernel", "decluster_kernel",
-                "interleave_kernel", "widen_velocity_kernel", "sl_multistep_kernel"):
+                "relayout_kernel", "sl_multistep_kernel"):
         if tok in base:
             tmpl = base[base.find("<"):base.find(">") + 1] if "<" in base and tok == "idw_kernel" else ""
             return tok + tmpl

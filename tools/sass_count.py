@@ -1,5 +1,5 @@
 """Instruction mix of a kernel's hottest loop from the SASS of libpysteps_b200.so:
-    python tools/sass_count.py sl_multistep_kernelIfLb1ELi4
+    python tools/sass_count.py sl_multistep_kernelIfLb1ELb0
 Finds the innermost backward branch with the largest body and counts its instructions by pipe."""
 import re
 import subprocess
