@@ -494,6 +494,27 @@ int b200_darts_normal(const double *spectrum, int N_x, int N_y, int N_t, int M_x
 int b200_darts_synthesize(const double *coef, int h, int w, const double *ey, const double *ex, int m, int n,
                           double *out, void *stream);
 
+/* ------------------------------------------------------------------------
+ * Local Lagrangian probability nowcast (pysteps/nowcasts/lagrangian_probability.py): the
+ * exceedance probability of every lead time's extrapolated field in a disk neighbourhood whose
+ * diameter grows with lead time.  The reference convolves with scipy's FFT; these counts are exact.
+ * ---------------------------------------------------------------------- */
+#define B200_PROBABILITY_MAX_SCALE (1 << 24) /* largest kernel diameter s */
+
+/* field: T planes (m, n) of `dtype` on the device, plane t at field + t * plane_stride elements
+ * (plane_stride 0: one field for every lead).  A NaN pixel is invalid and counts as an exceedance
+ * when nan_exceeds != 0; any other pixel v is valid and exceeds when (double)v >= threshold.
+ * scales (HOST, T entries): the kernel diameter s of each lead.  runs (device int32): for the leads
+ * with s > 0 in order, s pairs (b0, b1) each -- kernel row a covers columns b0..b1 -- so that
+ *   count(y, x) = sum_a sum_{b0(a) <= b <= b1(a)} A(y + c - a, x + c - b),  c = (s - 1) / 2,
+ * pixels outside the frame counting zero (scipy.signal.convolve mode="same").  out (T, m, n) float64:
+ * NaN at invalid pixels; else the exceedance (0 or 1) for s == 0 and min(count(exceeds) /
+ * count(valid), 1) for s > 0, from exact 32-bit counts.  scratch: m (n + 1) 64-bit words on the
+ * device, reused by every lead.  m n < 2^31 and max(m, n) + s < 2^31.  Only enqueues kernels. */
+int b200_probability(const void *field, int dtype, int64_t plane_stride, int T, int m, int n,
+                     double threshold, int nan_exceeds, const int *scales, const int *runs,
+                     unsigned long long *scratch, double *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

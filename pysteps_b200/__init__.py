@@ -5,6 +5,7 @@ Drop-in replacements, behind pysteps' own ``get_method()`` registries, for
   * ``pysteps.motion.lucaskanade.dense_lucaskanade``
   * ``pysteps.motion.vet.vet``
   * ``pysteps.noise.motion.initialize_bps`` / ``generate_bps`` (fused into the advection call)
+  * ``pysteps.nowcasts.lagrangian_probability.forecast``
 Host code is Python; every array operation is a hand-written CUDA kernel in
 ``libpysteps_b200.so`` reached through ctypes (``include/pysteps_b200.h``).
 There is no CPU fallback: without the built library and a GPU, calls raise.
@@ -14,4 +15,5 @@ __version__ = "0.1.0"
 from . import extrapolation  # noqa: F401
 from . import motion  # noqa: F401
 from . import noise  # noqa: F401
+from . import nowcasts  # noqa: F401
 from .interface import register  # noqa: F401

@@ -5,6 +5,8 @@ pysteps has no entry-point discovery for motion / extrapolation methods; the
   pysteps/extrapolation/interface.py:107-111  ``_extrapolation_methods``
   pysteps/motion/interface.py:36-46           ``_methods``
   pysteps/noise/interface.py:24-45            ``_noise_methods``  ("bps": the velocity perturbator)
+  pysteps/nowcasts/interface.py:44-54         ``_nowcast_methods`` ("probability": the local
+                                              Lagrangian probability nowcast)
 ``register()`` inserts the B200 callables under new names and, on request,
 under the stock names so that ``nowcasts.steps`` (which fetches the
 extrapolator by name at pysteps/nowcasts/steps.py:656 and
@@ -17,9 +19,12 @@ def methods():
     from .extrapolation import semilagrangian
 
     from .noise import motion as bps
+    from .nowcasts import lagrangian_probability
 
     out = {"extrapolation": {"semilagrangian_b200": semilagrangian.extrapolate}, "motion": {},
-           "noise": {"bps_b200": (bps.initialize_bps, bps.generate_bps)}}
+           "noise": {"bps_b200": (bps.initialize_bps, bps.generate_bps)},
+           "nowcasts": {"lagrangian_probability_b200": lagrangian_probability.forecast,
+                        "probability_b200": lagrangian_probability.forecast}}
     try:
         from .motion import lucaskanade
         out["motion"]["lk_b200"] = lucaskanade.dense_lucaskanade
@@ -46,12 +51,14 @@ def register(override=False):
     override=False: only the ``*_b200`` names are added (the identity checks of
     pysteps/tests/test_interfaces.py keep passing).  override=True additionally
     replaces ``"semilagrangian"``, ``"lk"``/``"lucaskanade"``, ``"vet"``, ``"proesmans"``,
-    ``"constant"``, ``"darts"`` and the noise method ``"bps"``.
+    ``"constant"``, ``"darts"``, the noise method ``"bps"`` and the nowcasts ``"probability"`` /
+    ``"lagrangian_probability"``.
     Returns the list of registered names.
     """
     import pysteps.extrapolation.interface as ei
     import pysteps.motion.interface as mi
     import pysteps.noise.interface as ni
+    import pysteps.nowcasts.interface as nci
 
     done = []
     m = methods()
@@ -73,4 +80,10 @@ def register(override=False):
         if override:
             ni._noise_methods[name.replace("_b200", "")] = fns
             done.append("noise:" + name.replace("_b200", ""))
+    for name, fn in m["nowcasts"].items():
+        nci._nowcast_methods[name] = fn
+        done.append("nowcasts:" + name)
+        if override:
+            nci._nowcast_methods[name.replace("_b200", "")] = fn
+            done.append("nowcasts:" + name.replace("_b200", ""))
     return done
