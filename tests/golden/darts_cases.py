@@ -7,6 +7,7 @@ from pysteps_b200 import _synthetic as syn
 CASES = [
     "shift_256_f64", "shift_256_f32", "shift_2048_f64", "t9_nt6_192x160", "alias_80x90", "odd_97x131",
     "small_64x48", "lsq1_128x128", "spectral_128x112", "rotation_160x160", "all_equal_96x96", "masked_nan_128x96",
+    "m5_256x224", "fx_tiles_160x256", "t2_nt0_96x80", "alias_fill_12x9",
 ]
 
 # The golden keeps the file small without losing the field: the reference's field is
@@ -64,6 +65,14 @@ def build_case(name):
         mask = np.zeros(R.shape, bool)
         mask[2, 5:25, 5:40] = True
         return np.ma.MaskedArray(R, mask=mask), kw
+    if name == "m5_256x224":  # the most unknowns supported: n_c = 242
+        return syn.rain_frames(256, 224, 6, seed=29, dx=2, dy=1), dict(kw, N_x=30, N_y=30, M_x=5, M_y=5)
+    if name == "fx_tiles_160x256":  # fx = 73: a second 64-wide frequency tile of the x pass
+        return syn.rain_frames(160, 256, 6, seed=30, dx=-2, dy=2), dict(kw, N_x=70, M_x=2, N_y=20)
+    if name == "t2_nt0_96x80":  # T = 2 admits only N_t = 0; y = k_t X is then zero, so is the field: MM holds
+        return syn.rain_frames(96, 80, 2, seed=31, dx=1, dy=1), dict(kw, N_t=0)
+    if name == "alias_fill_12x9":  # M_x = 5 on n = 9: _fill puts several coefficients on one column
+        return syn.rain_frames(12, 9, 4, seed=32, dx=1, dy=0), dict(kw, N_t=1, N_x=2, N_y=3, M_x=5, M_y=2)
     raise KeyError(name)
 
 
