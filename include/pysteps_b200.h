@@ -515,6 +515,39 @@ int b200_probability(const void *field, int dtype, int64_t plane_stride, int T, 
                      double threshold, int nan_exceeds, const int *scales, const int *runs,
                      unsigned long long *scratch, double *out, void *stream);
 
+/* ------------------------------------------------------------------------
+ * Ensemble statistics (pysteps/postprocessing/ensemblestats.py): reductions over the member axis of
+ * a (k, N) ensemble X of `dtype` on the device, member i at X + i * N elements, N < 2^31 pixels.
+ * flags (device int, zeroed by the call): the warnings NumPy raises, as bits. */
+#define B200_ENSEMBLE_OVERFLOW 1 /* a sum overflowed: "overflow encountered in reduce" */
+#define B200_ENSEMBLE_INVALID 2  /* a sum met inf + -inf: "invalid value encountered in reduce" */
+#define B200_ENSEMBLE_EMPTY 4    /* a pixel had no member to average: "Mean of empty slice" */
+
+/* out (N) of `dtype`.  nan_mode 0: np.mean -- the sequential sum over members in `dtype`, divided
+ * by k.  nan_mode 1: np.nanmean -- members that are NaN, or below thr when use_thr (compared in
+ * double; thr is already rounded to NumPy's comparison dtype), add 0 and are not counted; out =
+ * (dtype)((double)sum / count).  Only enqueues kernels. */
+int b200_ensemble_mean(const void *X, int dtype, int k, int64_t N, int nan_mode, int use_thr, double thr,
+                       void *out, int *flags, void *stream);
+
+/* out (n_thr, N) float64: for every threshold thr[t] (HOST array) the exact count c of members with
+ * finite X >= thr[t]; c / k, or NaN where a member is not finite (ignore_nan 0), or c / the number of
+ * finite members (ignore_nan 1).  Only enqueues kernels. */
+int b200_ensemble_excprob(const void *X, int dtype, int k, int64_t N, const double *thr, int n_thr,
+                          int ignore_nan, double *out, int *flags, void *stream);
+
+/* Band depth, step 1: the mask of the pixels whose members are all finite and some member >= thr,
+ * col (N int32): the pixel's column among the masked pixels in C order, -1 elsewhere; *p (device
+ * int64): the number of masked pixels.  Only enqueues kernels. */
+int b200_ensemble_band_mask(const void *X, int dtype, int k, int64_t N, double thr, int *col, int64_t *p,
+                            void *stream);
+
+/* Band depth, step 2: b (k, p) float64 tie-breaks; at every masked pixel member i has the rank
+ * r = 1 + #{j : X_j < X_i, or X_j == X_i and (b_j < b_i, or b_j == b_i and j < i)}; match (k
+ * int64): the sum of (k - r) (r - 1) over the masked pixels.  Only enqueues kernels. */
+int b200_ensemble_band_match(const void *X, int dtype, int k, int64_t N, const int *col, const double *b,
+                             int64_t p, int64_t *match, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

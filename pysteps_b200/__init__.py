@@ -6,6 +6,7 @@ Drop-in replacements, behind pysteps' own ``get_method()`` registries, for
   * ``pysteps.motion.vet.vet``
   * ``pysteps.noise.motion.initialize_bps`` / ``generate_bps`` (fused into the advection call)
   * ``pysteps.nowcasts.lagrangian_probability.forecast``
+  * ``pysteps.postprocessing.ensemblestats.mean`` / ``excprob`` / ``banddepth``
 Host code is Python; every array operation is a hand-written CUDA kernel in
 ``libpysteps_b200.so`` reached through ctypes (``include/pysteps_b200.h``).
 There is no CPU fallback: without the built library and a GPU, calls raise.
@@ -16,4 +17,5 @@ from . import extrapolation  # noqa: F401
 from . import motion  # noqa: F401
 from . import noise  # noqa: F401
 from . import nowcasts  # noqa: F401
+from . import postprocessing  # noqa: F401
 from .interface import register  # noqa: F401

@@ -121,6 +121,13 @@ _SIGNATURES = {
     "b200_convert":(c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p]),
     "b200_probability": (c_int, [c_void_p, c_int, c_i64, c_int, c_int, c_int, c_double, c_int,
                                  ctypes.POINTER(c_int), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_ensemble_mean": (c_int, [c_void_p, c_int, c_int, c_i64, c_int, c_int, c_double, c_void_p, c_void_p,
+                                   c_void_p]),
+    "b200_ensemble_excprob": (c_int, [c_void_p, c_int, c_int, c_i64, c_dp, c_int, c_int, c_void_p, c_void_p,
+                                      c_void_p]),
+    "b200_ensemble_band_mask": (c_int, [c_void_p, c_int, c_int, c_i64, c_double, c_void_p, c_void_p, c_void_p]),
+    "b200_ensemble_band_match": (c_int, [c_void_p, c_int, c_int, c_i64, c_void_p, c_void_p, c_i64, c_void_p,
+                                         c_void_p]),
 }
 
 

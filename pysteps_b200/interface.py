@@ -7,6 +7,8 @@ pysteps has no entry-point discovery for motion / extrapolation methods; the
   pysteps/noise/interface.py:24-45            ``_noise_methods``  ("bps": the velocity perturbator)
   pysteps/nowcasts/interface.py:44-54         ``_nowcast_methods`` ("probability": the local
                                               Lagrangian probability nowcast)
+  pysteps/postprocessing/interface.py:29-33   ``_ensemblestats_methods`` ("mean", "excprob",
+                                              "banddepth")
 ``register()`` inserts the B200 callables under new names and, on request,
 under the stock names so that ``nowcasts.steps`` (which fetches the
 extrapolator by name at pysteps/nowcasts/steps.py:656 and
@@ -20,11 +22,14 @@ def methods():
 
     from .noise import motion as bps
     from .nowcasts import lagrangian_probability
+    from .postprocessing import ensemblestats
 
     out = {"extrapolation": {"semilagrangian_b200": semilagrangian.extrapolate}, "motion": {},
            "noise": {"bps_b200": (bps.initialize_bps, bps.generate_bps)},
            "nowcasts": {"lagrangian_probability_b200": lagrangian_probability.forecast,
-                        "probability_b200": lagrangian_probability.forecast}}
+                        "probability_b200": lagrangian_probability.forecast},
+           "ensemblestats": {"mean_b200": ensemblestats.mean, "excprob_b200": ensemblestats.excprob,
+                             "banddepth_b200": ensemblestats.banddepth}}
     try:
         from .motion import lucaskanade
         out["motion"]["lk_b200"] = lucaskanade.dense_lucaskanade
@@ -51,14 +56,17 @@ def register(override=False):
     override=False: only the ``*_b200`` names are added (the identity checks of
     pysteps/tests/test_interfaces.py keep passing).  override=True additionally
     replaces ``"semilagrangian"``, ``"lk"``/``"lucaskanade"``, ``"vet"``, ``"proesmans"``,
-    ``"constant"``, ``"darts"``, the noise method ``"bps"`` and the nowcasts ``"probability"`` /
-    ``"lagrangian_probability"``.
+    ``"constant"``, ``"darts"``, the noise method ``"bps"``, the nowcasts ``"probability"`` /
+    ``"lagrangian_probability"`` and the ensemble statistics ``"mean"``, ``"excprob"`` and
+    ``"banddepth"``.  Only the registries change: ``from pysteps.postprocessing.ensemblestats import
+    excprob`` (and every other direct import) still gives the stock function.
     Returns the list of registered names.
     """
     import pysteps.extrapolation.interface as ei
     import pysteps.motion.interface as mi
     import pysteps.noise.interface as ni
     import pysteps.nowcasts.interface as nci
+    import pysteps.postprocessing.interface as ppi
 
     done = []
     m = methods()
@@ -86,4 +94,10 @@ def register(override=False):
         if override:
             nci._nowcast_methods[name.replace("_b200", "")] = fn
             done.append("nowcasts:" + name.replace("_b200", ""))
+    for name, fn in m["ensemblestats"].items():
+        ppi._ensemblestats_methods[name] = fn
+        done.append("ensemblestats:" + name)
+        if override:
+            ppi._ensemblestats_methods[name.replace("_b200", "")] = fn
+            done.append("ensemblestats:" + name.replace("_b200", ""))
     return done

@@ -21,7 +21,7 @@ tests/test_host_logic_probability.py (oracle and host logic on the CPU).
 import numpy as np
 import torch
 
-from .. import _device, _lib
+from .. import _compare, _device, _lib
 from ..extrapolation import interface as _extrapolation
 from ..extrapolation import semilagrangian as _sl
 from ..noise import motion as _bps
@@ -116,11 +116,7 @@ def _threshold_rule(dtype, threshold):
     fill = np.zeros(1, dtype=dt)
     fill[0] = threshold - 1
     nan_exceeds = bool((fill >= threshold)[0])
-    ct = np.result_type(fill, threshold)
-    if ct not in (np.float32, np.float64):
-        raise NotImplementedError(f"pysteps_b200 lagrangian_probability: a threshold of type {type(threshold)} "
-                                  "is not supported")
-    return float(np.asarray(threshold).astype(ct)), nan_exceeds
+    return _compare.comparison_threshold(dt, threshold, "lagrangian_probability")[0], nan_exceeds
 
 
 def _scales(timesteps, slope, side):
