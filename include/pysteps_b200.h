@@ -548,6 +548,62 @@ int b200_ensemble_band_mask(const void *X, int dtype, int k, int64_t N, double t
 int b200_ensemble_band_match(const void *X, int dtype, int k, int64_t N, const int *col, const double *b,
                              int64_t p, int64_t *match, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Linear and salient blending (pysteps/blending/linear_blending.py).  All arrays are device memory
+ * unless stated otherwise; dtypes are B200_F32 / B200_F64. */
+#define B200_BLEND_COPY 0   /* transform None */
+#define B200_BLEND_SQUARE 1 /* "sqrt": x**2 */
+#define B200_BLEND_DB 2     /* "dB": 10**(x/10) */
+#define B200_BLEND_EXP 3    /* "BoxCox"/"log", lambda 0: exp(x) */
+#define B200_BLEND_BOXCOX 4 /* "BoxCox"/"log": exp(log(lambda x + 1) / lambda) */
+#define B200_BLEND_MM 1     /* unit "mm": x / a * b */
+#define B200_BLEND_DBZ 2    /* unit "dBZ": (x / a) ** b */
+#define B200_BLEND_NOWCAST 0 /* lead modes of b200_blend_linear */
+#define B200_BLEND_NWP 1
+#define B200_BLEND_LINEAR 2
+#define B200_BLEND_SKIP 3
+
+/* y (n) = the inverse transform `kind` of x (n) in the dtype, then y < thr -> zero for the
+ * transcendental kinds.  A pixel whose value lies within the kernel's error bound of thr is left
+ * unthresholded and appended to (fix_idx, fix_x) (its index and input value, in no fixed order, at
+ * most cap of them); *nfix (device) is their number, which may exceed cap.  The exact kinds take
+ * nfix = NULL. */
+int b200_blend_transform(const void *x, void *y, int dtype, int64_t n, int kind, double lam, double thr,
+                         double zero, long long *fix_idx, double *fix_x, int64_t cap, unsigned long long *nfix,
+                         void *stream);
+
+/* y (n) = x / a * b (B200_BLEND_MM) or (x / a) ** b (B200_BLEND_DBZ), a and b cast to the dtype; y may be x. */
+int b200_blend_unit(const void *x, void *y, int dtype, int64_t n, int kind, double a, double b, void *stream);
+
+/* y[idx[i]] = val[i] cast to the dtype, for i < n. */
+int b200_blend_scatter(void *y, int dtype, const long long *idx, const double *val, int64_t n, void *stream);
+
+/* out (n_out, T, P) of nwp_dtype.  Output member e reads nowcast member now_map[e] at
+ * now + now_map[e] * now_member + lead * P and NWP member nwp_map[e] likewise; the NWP is
+ * nan_to_num'd and a NaN of the nowcast becomes the NWP value (fill_nwp) or 0.  Per lead (device
+ * arrays of T): mode (B200_BLEND_*), bits (1: w_nwp * nwp in float64, 2: w_now * now in float64,
+ * 4: their sum in float64; otherwise in float32), w_nwp and w_now. */
+int b200_blend_linear(const void *now, int now_dtype, const int *now_map, int64_t now_member, const void *nwp,
+                      int nwp_dtype, const int *nwp_map, int64_t nwp_member, void *out, int n_out, int T, int64_t P,
+                      const int *mode, const int *bits, const double *w_nwp, const double *w_now, int fill_nwp,
+                      void *stream);
+
+/* Device scratch of b200_blend_salient and b200_dense_rank for a slab of n < 2^31 values. */
+int b200_blend_scratch_bytes(int64_t n, int64_t *bytes);
+
+/* One lead of the salient blend, written to out[:, lead] (layout of b200_blend_linear): the dense
+ * rank of diff over the (n_out, P) slab and _get_ws with w = weight, w1 = 1 - weight,
+ * w2 = weight**2, w12 = (1 - weight)**2.  n_out * P < 2^31.  Reads nothing back. */
+int b200_blend_salient(const void *now, int now_dtype, const int *now_map, int64_t now_member, const void *nwp,
+                       int nwp_dtype, const int *nwp_map, int64_t nwp_member, void *out, int n_out, int T,
+                       int64_t P, int lead, double w, double w1, double w2, double w12, int fill_nwp, void *scratch,
+                       int64_t scratch_bytes, void *stream);
+
+/* rank (n uint32): the dense rank (1-based) of every x, -0.0 equal to +0.0; *max_rank the largest;
+ * *nan_flag 1 when some x is NaN (the ranks are then meaningless).  n < 2^31. */
+int b200_dense_rank(const void *x, int dtype, int64_t n, unsigned *rank, unsigned *max_rank, int *nan_flag,
+                    void *scratch, int64_t scratch_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

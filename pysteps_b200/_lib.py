@@ -128,6 +128,17 @@ _SIGNATURES = {
     "b200_ensemble_band_mask": (c_int, [c_void_p, c_int, c_int, c_i64, c_double, c_void_p, c_void_p, c_void_p]),
     "b200_ensemble_band_match": (c_int, [c_void_p, c_int, c_int, c_i64, c_void_p, c_void_p, c_i64, c_void_p,
                                          c_void_p]),
+    "b200_blend_transform": (c_int, [c_void_p, c_void_p, c_int, c_i64, c_int, c_double, c_double, c_double,
+                                     c_void_p, c_void_p, c_i64, c_void_p, c_void_p]),
+    "b200_blend_unit": (c_int, [c_void_p, c_void_p, c_int, c_i64, c_int, c_double, c_double, c_void_p]),
+    "b200_blend_scatter": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_i64, c_void_p]),
+    "b200_blend_linear": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_void_p, c_int, c_void_p, c_i64, c_void_p,
+                                  c_int, c_int, c_i64, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "b200_blend_scratch_bytes": (c_int, [c_i64, ctypes.POINTER(c_i64)]),
+    "b200_blend_salient": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_void_p, c_int, c_void_p, c_i64, c_void_p,
+                                   c_int, c_int, c_i64, c_int, c_double, c_double, c_double, c_double, c_int,
+                                   c_void_p, c_i64, c_void_p]),
+    "b200_dense_rank": (c_int, [c_void_p, c_int, c_i64, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p]),
 }
 
 

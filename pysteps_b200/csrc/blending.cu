@@ -1,0 +1,682 @@
+// blending.cu -- linear and salient blending of pysteps/blending/linear_blending.py on the device
+// (sm_90a).
+//   transform  the inverse transforms of utils/conversion.py:to_rainrate in the field's dtype; the
+//              exact ones (copy, square) bit for bit, the transcendental ones (10**(x/10), exp, the
+//              Box-Cox inverse) within a few ulp.  Every pixel whose value lies within the error
+//              bound of the threshold goes to a list (index, input value) that the host settles
+//              with NumPy's own expression; every other pixel is decided here.
+//   unit       mm -> mm/h (x / a * b, exact) and dBZ -> mm/h ((x / a) ** b) in place.
+//   linear     one launch for all leads and output members: the nowcast and NWP values are read
+//              through the member maps, the NWP is nan_to_num'd, the nowcast's NaN filled per output
+//              member, and each lead copied or blended in the dtypes the host passes (no FMA).
+//   salient    per lead: maxima of both slabs (integer atomics on order-preserving keys), diff and
+//              its 64-bit keys, an LSD radix sort of (key, index) pairs in 8-bit digits that skips
+//              every digit all keys share, a dense rank from an inclusive scan of key changes
+//              scattered back to pixel order, then the salience weight and the blended value.
+// No atomics touch floating-point values and every scan runs in a fixed order, so repeated calls
+// are bit-identical.
+#include <algorithm>
+
+#include "common.cuh"
+
+namespace {
+
+constexpr int THREADS = 256;
+constexpr int SORT_ITEMS = 16;
+constexpr int TILE = THREADS * SORT_ITEMS;  // keys per radix tile and per scan block
+constexpr int RADIX = 256;
+constexpr int PASSES = 8;
+constexpr unsigned FULL = 0xffffffffu;
+
+__device__ __forceinline__ double quiet_nan() { return __longlong_as_double(0x7ff8000000000000ll); }
+
+template <typename T> __device__ __forceinline__ T max_finite();
+template <> __device__ __forceinline__ float max_finite<float>() { return 3.4028234663852886e38f; }
+template <> __device__ __forceinline__ double max_finite<double>() { return 1.7976931348623157e308; }
+
+// np.nan_to_num: NaN -> 0, +-inf -> +-max finite of the dtype
+template <typename T> __device__ __forceinline__ T nan_to_num(T v) {
+    if (isnan(v)) return T(0);
+    if (isinf(v)) return v > T(0) ? max_finite<T>() : -max_finite<T>();
+    return v;
+}
+
+// order-preserving 64-bit image of a double; -0.0 maps to +0.0 (rankdata treats them as equal)
+__device__ __forceinline__ unsigned long long order_key(double d) {
+    unsigned long long u = (unsigned long long)__double_as_longlong(d == 0.0 ? 0.0 : d);
+    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double key_value(unsigned long long k) {
+    if (k == ~0ull) return quiet_nan();
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+// ---------------------------------------------------------------- conversion to rain rate
+template <typename T>
+__global__ void __launch_bounds__(THREADS)
+    transform_kernel(const T *__restrict__ x, T *__restrict__ y, int64_t n, int kind, double lam, double thr,
+                     double zero, double eps, long long *__restrict__ fix_idx, double *__restrict__ fix_x,
+                     long long cap, unsigned long long *__restrict__ nfix) {
+    for (int64_t i = (int64_t)blockIdx.x * THREADS + threadIdx.x; i < n; i += (int64_t)gridDim.x * THREADS) {
+        const T v = x[i];
+        T r;
+        double rel = 0.0;
+        if (kind == B200_BLEND_COPY) {
+            r = v;
+        } else if (kind == B200_BLEND_SQUARE) {
+            r = v * v;
+        } else if (kind == B200_BLEND_DB) {
+            r = pow(T(10), v / T(10));
+            rel = 16.0 * eps;
+        } else if (kind == B200_BLEND_EXP) {
+            r = exp(v);
+            rel = 16.0 * eps;
+        } else {  // Box-Cox, lambda != 0: exp(log(lambda x + 1) / lambda), the error grows with the exponent
+            const T z = log(T(lam) * v + T(1)) / T(lam);
+            r = exp(z);
+            rel = 16.0 * eps * (2.0 + fabs((double)z));
+        }
+        if (rel > 0.0) {
+            const double d = (double)r;
+            // a non-finite value is never within the bound of a finite threshold
+            if (isfinite(d) && fabs(d - thr) <= rel * fmax(fabs(d), fabs(thr)) + 1e-300) {
+                const unsigned long long slot = atomicAdd(nfix, 1ull);
+                if ((long long)slot < cap) {
+                    fix_idx[slot] = i;
+                    fix_x[slot] = (double)v;
+                }
+            } else if (d < thr) {
+                r = (T)zero;
+            }
+        }
+        y[i] = r;
+    }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(THREADS) unit_kernel(const T *x, T *y, int64_t n, int kind, double a, double b) {
+    for (int64_t i = (int64_t)blockIdx.x * THREADS + threadIdx.x; i < n; i += (int64_t)gridDim.x * THREADS) {
+        const T v = x[i];
+        y[i] = kind == B200_BLEND_MM ? v / T(a) * T(b) : pow(v / T(a), T(b));
+    }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(THREADS)
+    scatter_kernel(T *__restrict__ y, const long long *__restrict__ idx, const double *__restrict__ val, int64_t n) {
+    const int64_t i = (int64_t)blockIdx.x * THREADS + threadIdx.x;
+    if (i < n) y[idx[i]] = (T)val[i];
+}
+
+// ---------------------------------------------------------------- the member-mapped fields
+struct Fields {
+    const void *now;
+    const int *now_map;
+    int64_t now_member;
+    const void *nwp;
+    const int *nwp_map;
+    int64_t nwp_member;
+    int64_t P;
+    int fill_nwp;
+};
+
+// the nowcast value of output member e at lead i, pixel p, its NaN filled as the reference does
+template <typename Tc, typename Tn>
+__device__ __forceinline__ Tc now_value(const Fields &f, int e, int i, int64_t p) {
+    Tc v = ((const Tc *)f.now)[(int64_t)f.now_map[e] * f.now_member + (int64_t)i * f.P + p];
+    if (isnan(v)) {
+        const Tn w = ((const Tn *)f.nwp)[(int64_t)f.nwp_map[e] * f.nwp_member + (int64_t)i * f.P + p];
+        v = f.fill_nwp ? (Tc)nan_to_num(w) : Tc(0);
+    }
+    return v;
+}
+template <typename Tn>
+__device__ __forceinline__ Tn nwp_value(const Fields &f, int e, int i, int64_t p) {
+    return nan_to_num(((const Tn *)f.nwp)[(int64_t)f.nwp_map[e] * f.nwp_member + (int64_t)i * f.P + p]);
+}
+
+template <typename T> __device__ __forceinline__ T mul(double w, T v) { return T(w) * v; }
+
+// modes: B200_BLEND_NOWCAST, B200_BLEND_NWP, B200_BLEND_LINEAR (dtype bits: 1 w_nwp * nwp in float64,
+// 2 w_now * now in float64, 4 their sum in float64), B200_BLEND_SKIP
+template <typename Tc, typename Tn>
+__global__ void __launch_bounds__(THREADS)
+    linear_kernel(Fields f, Tn *__restrict__ out, int n_out, int T, const int *__restrict__ mode,
+                  const int *__restrict__ bits, const double *__restrict__ w_nwp, const double *__restrict__ w_now) {
+    for (int y = blockIdx.y; y < n_out * T; y += gridDim.y) {
+        const int e = y / T, i = y % T, md = mode[i];
+        if (md == B200_BLEND_SKIP) continue;
+        const int bt = bits[i];
+        const double wn = w_nwp[i], wc = w_now[i];
+        Tn *o = out + (int64_t)y * f.P;
+        for (int64_t p = (int64_t)blockIdx.x * THREADS + threadIdx.x; p < f.P; p += (int64_t)gridDim.x * THREADS) {
+            if (md == B200_BLEND_NOWCAST) {
+                o[p] = (Tn)now_value<Tc, Tn>(f, e, i, p);
+            } else if (md == B200_BLEND_NWP) {
+                o[p] = nwp_value<Tn>(f, e, i, p);
+            } else {
+                const Tn g = nwp_value<Tn>(f, e, i, p);
+                const Tc c = now_value<Tc, Tn>(f, e, i, p);
+                const double a = (bt & 1) ? wn * (double)g : (double)mul<Tn>(wn, g);
+                const double b = (bt & 2) ? wc * (double)c : (double)mul<Tc>(wc, c);
+                o[p] = (bt & 4) ? (Tn)(a + b) : (Tn)((float)a + (float)b);
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------- salience: maxima, diff, keys
+struct SortScratch {
+    unsigned long long *key[2];
+    unsigned *idx[2];
+    unsigned *tiles;  // RADIX x n_tiles digit counts, digit-major, then their exclusive scan
+    unsigned *bsum;   // per scan block sums
+    unsigned *rank;   // dense rank of every pixel
+    unsigned *ghist;  // PASSES x RADIX global digit counts
+    int *src;         // PASSES + 1: buffer each pass reads (-1: pass skipped); [PASSES]: the final buffer
+    unsigned long long *maxkey;  // 2: maxima of the two slabs
+    int *nan_flag;
+    unsigned *max_rank;
+};
+
+static int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
+
+static int64_t carve(SortScratch *s, char *base, int64_t n) {
+    const int64_t n_tiles = b200::ceil_div64(std::max<int64_t>(n, 1), TILE);
+    const int64_t n_scan = std::max<int64_t>(RADIX * n_tiles, n);
+    const int64_t n_bsum = b200::ceil_div64(n_scan, TILE);
+    int64_t off = 0;
+    auto take = [&](int64_t bytes) {
+        char *p = base ? base + off : nullptr;
+        off += align256(bytes);
+        return p;
+    };
+    s->key[0] = (unsigned long long *)take(8 * n);
+    s->key[1] = (unsigned long long *)take(8 * n);
+    s->idx[0] = (unsigned *)take(4 * n);
+    s->idx[1] = (unsigned *)take(4 * n);
+    s->tiles = (unsigned *)take(4 * RADIX * n_tiles);
+    s->bsum = (unsigned *)take(4 * n_bsum);
+    s->rank = (unsigned *)take(4 * n);
+    s->ghist = (unsigned *)take(4 * PASSES * RADIX);
+    s->src = (int *)take(4 * (PASSES + 1));
+    s->maxkey = (unsigned long long *)take(16);
+    s->nan_flag = (int *)take(4);
+    s->max_rank = (unsigned *)take(4);
+    return off;
+}
+
+// warp max of 64-bit values (no 64-bit redux instruction)
+__device__ __forceinline__ unsigned long long warp_max64(unsigned long long v) {
+    for (int o = 16; o; o >>= 1) v = max(v, (unsigned long long)__shfl_xor_sync(FULL, v, o));
+    return v;
+}
+
+template <typename Tc, typename Tn>
+__global__ void __launch_bounds__(THREADS) slab_max(Fields f, int n_out, int lead, unsigned long long *maxkey) {
+    unsigned long long mc = 0, mn = 0;
+    const int64_t n = (int64_t)n_out * f.P;
+    for (int64_t j = (int64_t)blockIdx.x * THREADS + threadIdx.x; j < n; j += (int64_t)gridDim.x * THREADS) {
+        const int e = (int)(j / f.P);
+        const int64_t p = j - (int64_t)e * f.P;
+        const Tc c = now_value<Tc, Tn>(f, e, lead, p);
+        const Tn g = nwp_value<Tn>(f, e, lead, p);
+        mc = max(mc, isnan(c) ? ~0ull : order_key((double)c));  // NaN propagates: the largest key
+        mn = max(mn, isnan(g) ? ~0ull : order_key((double)g));
+    }
+    mc = warp_max64(mc);
+    mn = warp_max64(mn);
+    if ((threadIdx.x & 31) == 0) {
+        atomicMax(maxkey, mc);
+        atomicMax(maxkey + 1, mn);
+    }
+}
+
+// diff = nowcast / max - nwp / max (zeros for a slab whose max == 0) in the reference's dtypes
+template <typename Tc, typename Tn, typename Td>
+__global__ void __launch_bounds__(THREADS)
+    diff_keys(Fields f, int n_out, int lead, const unsigned long long *__restrict__ maxkey,
+              unsigned long long *__restrict__ key, unsigned *__restrict__ idx, int *__restrict__ nan_flag) {
+    const Tc mc = (Tc)key_value(maxkey[0]);
+    const Tn mn = (Tn)key_value(maxkey[1]);
+    const int64_t n = (int64_t)n_out * f.P;
+    int nan_seen = 0;
+    for (int64_t j = (int64_t)blockIdx.x * THREADS + threadIdx.x; j < n; j += (int64_t)gridDim.x * THREADS) {
+        const int e = (int)(j / f.P);
+        const int64_t p = j - (int64_t)e * f.P;
+        const Tc c = mc == Tc(0) ? Tc(0) : now_value<Tc, Tn>(f, e, lead, p) / mc;
+        const Tn g = mn == Tn(0) ? Tn(0) : nwp_value<Tn>(f, e, lead, p) / mn;
+        const Td d = (Td)c - (Td)g;
+        nan_seen |= isnan(d);
+        key[j] = order_key((double)d);
+        idx[j] = (unsigned)j;
+    }
+    if (__any_sync(FULL, nan_seen) && (threadIdx.x & 31) == 0) atomicOr(nan_flag, 1);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(THREADS)
+    array_keys(const T *__restrict__ x, int64_t n, unsigned long long *__restrict__ key, unsigned *__restrict__ idx,
+               int *__restrict__ nan_flag) {
+    int nan_seen = 0;
+    for (int64_t j = (int64_t)blockIdx.x * THREADS + threadIdx.x; j < n; j += (int64_t)gridDim.x * THREADS) {
+        const double d = (double)x[j];
+        nan_seen |= isnan(d);
+        key[j] = order_key(d);
+        idx[j] = (unsigned)j;
+    }
+    if (__any_sync(FULL, nan_seen) && (threadIdx.x & 31) == 0) atomicOr(nan_flag, 1);
+}
+
+// ---------------------------------------------------------------- radix sort
+__global__ void __launch_bounds__(THREADS)
+    global_hist(const unsigned long long *__restrict__ key, int64_t n, unsigned *__restrict__ ghist) {
+    __shared__ unsigned h[PASSES][RADIX];
+    for (int t = threadIdx.x; t < PASSES * RADIX; t += THREADS) (&h[0][0])[t] = 0;
+    __syncthreads();
+    for (int64_t j = (int64_t)blockIdx.x * THREADS + threadIdx.x; j < n; j += (int64_t)gridDim.x * THREADS) {
+        const unsigned long long k = key[j];
+#pragma unroll
+        for (int d = 0; d < PASSES; d++) atomicAdd(&h[d][(k >> (8 * d)) & 255], 1u);
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < PASSES * RADIX; t += THREADS)
+        if ((&h[0][0])[t]) atomicAdd(ghist + t, (&h[0][0])[t]);
+}
+
+// src[d]: the buffer pass d reads, or -1 when every key has the same digit d (the pass is skipped)
+__global__ void plan_passes(const unsigned *__restrict__ ghist, int64_t n, int *__restrict__ src) {
+    if (threadIdx.x != 0) return;
+    int cur = 0;
+    for (int d = 0; d < PASSES; d++) {
+        bool trivial = false;
+        for (int b = 0; b < RADIX; b++) trivial |= (int64_t)ghist[d * RADIX + b] == n;
+        src[d] = trivial ? -1 : cur;
+        if (!trivial) cur ^= 1;
+    }
+    src[PASSES] = cur;
+}
+
+__global__ void __launch_bounds__(THREADS)
+    tile_hist(SortScratch s, int64_t n, int64_t n_tiles, int pass) {
+    const int b = s.src[pass];
+    if (b < 0) return;
+    __shared__ unsigned h[RADIX];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const unsigned long long *key = s.key[b];
+    const int64_t t0 = (int64_t)blockIdx.x * TILE;
+    for (int r = 0; r < SORT_ITEMS; r++) {
+        const int64_t j = t0 + r * THREADS + threadIdx.x;
+        if (j < n) atomicAdd(&h[(key[j] >> (8 * pass)) & 255], 1u);
+    }
+    __syncthreads();
+    s.tiles[(int64_t)threadIdx.x * n_tiles + blockIdx.x] = h[threadIdx.x];
+}
+
+// block-wide exclusive scan of one value per thread; returns the total in *total
+__device__ __forceinline__ unsigned block_exclusive(unsigned v, unsigned *total) {
+    __shared__ unsigned warp_sum[THREADS / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    unsigned x = v;
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned y = __shfl_up_sync(FULL, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_sum[w] = x;
+    __syncthreads();
+    if (w == 0) {
+        unsigned s = lane < THREADS / 32 ? warp_sum[lane] : 0;
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned y = __shfl_up_sync(FULL, s, o);
+            if (lane >= o) s += y;
+        }
+        if (lane < THREADS / 32) warp_sum[lane] = s;
+    }
+    __syncthreads();
+    const unsigned before = (w ? warp_sum[w - 1] : 0) + x - v;
+    *total = warp_sum[THREADS / 32 - 1];
+    __syncthreads();
+    return before;
+}
+
+// the scans: over the tile counts of a pass (exclusive, in place), or over the key changes of the
+// sorted keys (inclusive: the dense rank, scattered to pixel order)
+struct CountScan {
+    SortScratch s;
+    int pass;
+    __device__ bool skip() const { return s.src[pass] < 0; }
+    __device__ unsigned load(int64_t i) const { return s.tiles[i]; }
+    __device__ void store(int64_t i, unsigned excl, unsigned) const { s.tiles[i] = excl; }
+};
+struct RankScan {
+    SortScratch s;
+    int64_t n;
+    __device__ bool skip() const { return false; }
+    __device__ unsigned load(int64_t i) const {
+        const unsigned long long *k = s.key[s.src[PASSES]];
+        return i == 0 || k[i] != k[i - 1];
+    }
+    __device__ void store(int64_t i, unsigned excl, unsigned v) const {
+        const unsigned incl = excl + v;
+        s.rank[s.idx[s.src[PASSES]][i]] = incl;
+        if (i == n - 1) *s.max_rank = incl;
+    }
+};
+
+template <typename Op>
+__global__ void __launch_bounds__(THREADS) scan_reduce(Op op, int64_t n, unsigned *__restrict__ bsum) {
+    if (op.skip()) return;
+    const int64_t i0 = (int64_t)blockIdx.x * TILE + (int64_t)threadIdx.x * SORT_ITEMS;
+    unsigned v = 0;
+    for (int r = 0; r < SORT_ITEMS; r++)
+        if (i0 + r < n) v += op.load(i0 + r);
+    unsigned total;
+    block_exclusive(v, &total);
+    if (threadIdx.x == 0) bsum[blockIdx.x] = total;
+}
+
+template <typename Op>
+__global__ void __launch_bounds__(THREADS) scan_blocks(Op op, int64_t nb, unsigned *__restrict__ bsum) {
+    if (op.skip()) return;
+    unsigned carry = 0;
+    for (int64_t b0 = 0; b0 < nb; b0 += THREADS) {
+        const int64_t b = b0 + threadIdx.x;
+        const unsigned v = b < nb ? bsum[b] : 0;
+        unsigned total;
+        const unsigned e = block_exclusive(v, &total);
+        if (b < nb) bsum[b] = carry + e;
+        carry += total;
+    }
+}
+
+template <typename Op>
+__global__ void __launch_bounds__(THREADS) scan_apply(Op op, int64_t n, const unsigned *__restrict__ bsum) {
+    if (op.skip()) return;
+    const int64_t i0 = (int64_t)blockIdx.x * TILE + (int64_t)threadIdx.x * SORT_ITEMS;
+    unsigned v[SORT_ITEMS];
+    unsigned sum = 0;
+#pragma unroll
+    for (int r = 0; r < SORT_ITEMS; r++) {
+        v[r] = i0 + r < n ? op.load(i0 + r) : 0;
+        sum += v[r];
+    }
+    unsigned total;
+    unsigned run = bsum[blockIdx.x] + block_exclusive(sum, &total);
+#pragma unroll
+    for (int r = 0; r < SORT_ITEMS; r++) {
+        if (i0 + r < n) op.store(i0 + r, run, v[r]);
+        run += v[r];
+    }
+}
+
+// stable scatter of one tile: keys are taken in index order, ranked within their warp by
+// __match_any_sync and across the warps of a round by a per-digit scan in shared memory
+__global__ void __launch_bounds__(THREADS) scatter_pass(SortScratch s, int64_t n, int64_t n_tiles, int pass) {
+    const int b = s.src[pass];
+    if (b < 0) return;
+    __shared__ unsigned base[RADIX];
+    __shared__ unsigned wcnt[THREADS / 32][RADIX];
+    __shared__ unsigned round_total[RADIX];
+    const unsigned long long *ksrc = s.key[b];
+    const unsigned *isrc = s.idx[b];
+    unsigned long long *kdst = s.key[b ^ 1];
+    unsigned *idst = s.idx[b ^ 1];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    base[threadIdx.x] = s.tiles[(int64_t)threadIdx.x * n_tiles + blockIdx.x];
+    const int64_t t0 = (int64_t)blockIdx.x * TILE;
+    for (int r = 0; r < SORT_ITEMS; r++) {
+        for (int q = 0; q < THREADS / 32; q++) wcnt[q][threadIdx.x] = 0;
+        __syncthreads();
+        const int64_t j = t0 + (int64_t)r * THREADS + threadIdx.x;
+        const bool valid = j < n;
+        const unsigned long long k = valid ? ksrc[j] : 0ull;
+        const unsigned digit = valid ? (unsigned)((k >> (8 * pass)) & 255) : RADIX + lane;
+        const unsigned peers = __match_any_sync(FULL, digit);
+        const unsigned below = __popc(peers & ((1u << lane) - 1u));
+        if (valid && below == 0) wcnt[w][digit] = __popc(peers);
+        __syncthreads();
+        unsigned acc = 0;
+        for (int q = 0; q < THREADS / 32; q++) {
+            const unsigned c = wcnt[q][threadIdx.x];
+            wcnt[q][threadIdx.x] = acc;
+            acc += c;
+        }
+        round_total[threadIdx.x] = acc;
+        __syncthreads();
+        if (valid) {
+            const unsigned pos = base[digit] + wcnt[w][digit] + below;
+            kdst[pos] = k;
+            idst[pos] = isrc[j];
+        }
+        __syncthreads();
+        base[threadIdx.x] += round_total[threadIdx.x];
+    }
+}
+
+int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(b200::ceil_div64(n, THREADS), 132 * 16)); }
+
+// sort the n keys in s.key[0] / s.idx[0] and rank them densely into s.rank, s.max_rank
+int dense_rank(SortScratch &s, int64_t n, cudaStream_t st) {
+    const int64_t n_tiles = b200::ceil_div64(n, TILE);
+    B200_CUDA(cudaMemsetAsync(s.ghist, 0, 4 * PASSES * RADIX, st));
+    global_hist<<<grid_for(n), THREADS, 0, st>>>(s.key[0], n, s.ghist);
+    B200_LAUNCH_CHECK();
+    plan_passes<<<1, 32, 0, st>>>(s.ghist, n, s.src);
+    B200_LAUNCH_CHECK();
+    const int64_t n_counts = RADIX * n_tiles;
+    const int64_t nb = b200::ceil_div64(n_counts, TILE);
+    for (int d = 0; d < PASSES; d++) {
+        tile_hist<<<(unsigned)n_tiles, THREADS, 0, st>>>(s, n, n_tiles, d);
+        B200_LAUNCH_CHECK();
+        scan_reduce<<<(unsigned)nb, THREADS, 0, st>>>(CountScan{s, d}, n_counts, s.bsum);
+        B200_LAUNCH_CHECK();
+        scan_blocks<<<1, THREADS, 0, st>>>(CountScan{s, d}, nb, s.bsum);
+        B200_LAUNCH_CHECK();
+        scan_apply<<<(unsigned)nb, THREADS, 0, st>>>(CountScan{s, d}, n_counts, s.bsum);
+        B200_LAUNCH_CHECK();
+        scatter_pass<<<(unsigned)n_tiles, THREADS, 0, st>>>(s, n, n_tiles, d);
+        B200_LAUNCH_CHECK();
+    }
+    const int64_t rb = b200::ceil_div64(n, TILE);
+    scan_reduce<<<(unsigned)rb, THREADS, 0, st>>>(RankScan{s, n}, n, s.bsum);
+    B200_LAUNCH_CHECK();
+    scan_blocks<<<1, THREADS, 0, st>>>(RankScan{s, n}, rb, s.bsum);
+    B200_LAUNCH_CHECK();
+    scan_apply<<<(unsigned)rb, THREADS, 0, st>>>(RankScan{s, n}, n, s.bsum);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+// linear_blending.py:_get_ws on the dense rank, then ws * nowcast + (1 - ws) * nwp in float64;
+// w = weight, w1 = 1 - weight, w2 = weight**2, w12 = (1 - weight)**2 as the host computed them
+template <typename Tc, typename Tn>
+__global__ void __launch_bounds__(THREADS)
+    salient_kernel(Fields f, Tn *__restrict__ out, int n_out, int T, int lead, SortScratch s, double w, double w1,
+                   double w2, double w12) {
+    const int64_t n = (int64_t)n_out * f.P;
+    const bool all_nan = *s.nan_flag != 0;  // scipy's rankdata: one NaN makes every rank NaN
+    const double max_rank = (double)*s.max_rank;
+    for (int64_t j = (int64_t)blockIdx.x * THREADS + threadIdx.x; j < n; j += (int64_t)gridDim.x * THREADS) {
+        const int e = (int)(j / f.P);
+        const int64_t p = j - (int64_t)e * f.P;
+        double ws = quiet_nan();
+        if (!all_nan) {
+            const double r = (double)s.rank[j] / max_rank;
+            const double a = w * r;
+            const double q = 1.0 - r;
+            const double s1 = sqrt(r * r + w2);
+            const double s2 = sqrt(q * q + w12);
+            ws = 0.5 * (a / (a + w1 * q) + s1 / (s1 + s2));
+        }
+        const double v = ws * (double)now_value<Tc, Tn>(f, e, lead, p) + (1.0 - ws) * (double)nwp_value<Tn>(f, e, lead, p);
+        out[((int64_t)e * T + lead) * f.P + p] = (Tn)v;
+    }
+}
+
+template <typename T> int transform_run(const void *x, void *y, int64_t n, int kind, double lam, double thr,
+                                        double zero, long long *fix_idx, double *fix_x, long long cap,
+                                        unsigned long long *nfix, cudaStream_t st) {
+    const double eps = sizeof(T) == 4 ? 1.1920928955078125e-07 : 2.220446049250313e-16;
+    transform_kernel<T><<<grid_for(n), THREADS, 0, st>>>((const T *)x, (T *)y, n, kind, lam, thr, zero, eps, fix_idx,
+                                                        fix_x, cap, nfix);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+template <typename Tc, typename Tn>
+int linear_run(const Fields &f, void *out, int n_out, int T, const int *mode, const int *bits, const double *w_nwp,
+               const double *w_now, cudaStream_t st) {
+    const dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>(b200::ceil_div64(f.P, THREADS), 1024)),
+                    (unsigned)std::min(n_out * T, 65535));
+    linear_kernel<Tc, Tn><<<grid, THREADS, 0, st>>>(f, (Tn *)out, n_out, T, mode, bits, w_nwp, w_now);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+template <typename Tc, typename Tn, typename Td>
+int salient_run(const Fields &f, void *out, int n_out, int T, int lead, double w, double w1, double w2, double w12,
+                void *scratch, cudaStream_t st) {
+    const int64_t n = (int64_t)n_out * f.P;
+    SortScratch s;
+    carve(&s, (char *)scratch, n);
+    B200_CUDA(cudaMemsetAsync(s.maxkey, 0, 16, st));
+    B200_CUDA(cudaMemsetAsync(s.nan_flag, 0, 4, st));
+    slab_max<Tc, Tn><<<grid_for(n), THREADS, 0, st>>>(f, n_out, lead, s.maxkey);
+    B200_LAUNCH_CHECK();
+    diff_keys<Tc, Tn, Td><<<grid_for(n), THREADS, 0, st>>>(f, n_out, lead, s.maxkey, s.key[0], s.idx[0], s.nan_flag);
+    B200_LAUNCH_CHECK();
+    if (int rc = dense_rank(s, n, st)) return rc;
+    salient_kernel<Tc, Tn><<<grid_for(n), THREADS, 0, st>>>(f, (Tn *)out, n_out, T, lead, s, w, w1, w2, w12);
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int b200_blend_scratch_bytes(int64_t n, int64_t *bytes) {
+    B200_REQUIRE(n >= 0 && n < ((int64_t)1 << 31) && bytes != nullptr, "bad arguments");
+    SortScratch s;
+    *bytes = carve(&s, nullptr, n);
+    return 0;
+}
+
+extern "C" int b200_blend_transform(const void *x, void *y, int dtype, int64_t n, int kind, double lam, double thr,
+                                    double zero, long long *fix_idx, double *fix_x, int64_t cap,
+                                    unsigned long long *nfix, void *stream) {
+    B200_REQUIRE(n >= 0 && cap >= 0 && kind >= B200_BLEND_COPY && kind <= B200_BLEND_BOXCOX &&
+                     (kind < B200_BLEND_DB || nfix != nullptr),
+                 "bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (nfix) B200_CUDA(cudaMemsetAsync(nfix, 0, sizeof(unsigned long long), st));
+    if (n == 0) return 0;
+    B200_REQUIRE(x != nullptr && y != nullptr && (cap == 0 || (fix_idx != nullptr && fix_x != nullptr)),
+                 "bad arguments");
+    if (dtype == B200_F32) return transform_run<float>(x, y, n, kind, lam, thr, zero, fix_idx, fix_x, cap, nfix, st);
+    if (dtype == B200_F64) return transform_run<double>(x, y, n, kind, lam, thr, zero, fix_idx, fix_x, cap, nfix, st);
+    b200::set_error("blend_transform: dtype must be B200_F32 or B200_F64");
+    return B200_EINVAL;
+}
+
+extern "C" int b200_blend_unit(const void *x, void *y, int dtype, int64_t n, int kind, double a, double b,
+                               void *stream) {
+    B200_REQUIRE(n >= 0 && (kind == B200_BLEND_MM || kind == B200_BLEND_DBZ), "bad arguments");
+    if (n == 0) return 0;
+    B200_REQUIRE(x != nullptr && y != nullptr, "bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == B200_F32)
+        unit_kernel<float><<<grid_for(n), THREADS, 0, st>>>((const float *)x, (float *)y, n, kind, a, b);
+    else if (dtype == B200_F64)
+        unit_kernel<double><<<grid_for(n), THREADS, 0, st>>>((const double *)x, (double *)y, n, kind, a, b);
+    else {
+        b200::set_error("blend_unit: dtype must be B200_F32 or B200_F64");
+        return B200_EINVAL;
+    }
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int b200_blend_scatter(void *y, int dtype, const long long *idx, const double *val, int64_t n,
+                                  void *stream) {
+    B200_REQUIRE(n >= 0, "bad arguments");
+    if (n == 0) return 0;
+    B200_REQUIRE(y != nullptr && idx != nullptr && val != nullptr, "bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    const unsigned g = (unsigned)b200::ceil_div64(n, THREADS);
+    if (dtype == B200_F32) scatter_kernel<float><<<g, THREADS, 0, st>>>((float *)y, idx, val, n);
+    else if (dtype == B200_F64) scatter_kernel<double><<<g, THREADS, 0, st>>>((double *)y, idx, val, n);
+    else {
+        b200::set_error("blend_scatter: dtype must be B200_F32 or B200_F64");
+        return B200_EINVAL;
+    }
+    B200_LAUNCH_CHECK();
+    return 0;
+}
+
+static bool fields_ok(const void *now, const int *now_map, const void *nwp, const int *nwp_map, const void *out) {
+    return now && now_map && nwp && nwp_map && out;
+}
+
+extern "C" int b200_blend_linear(const void *now, int now_dtype, const int *now_map, int64_t now_member,
+                                 const void *nwp, int nwp_dtype, const int *nwp_map, int64_t nwp_member, void *out,
+                                 int n_out, int T, int64_t P, const int *mode, const int *bits, const double *w_nwp,
+                                 const double *w_now, int fill_nwp, void *stream) {
+    B200_REQUIRE(n_out >= 0 && T >= 0 && P >= 0 && (int64_t)n_out * T <= INT32_MAX, "bad arguments");
+    if ((int64_t)n_out * T * P == 0) return 0;
+    // now may be NULL when the nowcast has no lead (every lead is then B200_BLEND_NWP)
+    B200_REQUIRE(now_map && nwp && nwp_map && out && mode && bits && w_nwp && w_now, "bad arguments");
+    const Fields f{now, now_map, now_member, nwp, nwp_map, nwp_member, P, fill_nwp};
+    cudaStream_t st = (cudaStream_t)stream;
+    const int c = now_dtype * 2 + nwp_dtype;
+    if (c == 0) return linear_run<float, float>(f, out, n_out, T, mode, bits, w_nwp, w_now, st);
+    if (c == 1) return linear_run<float, double>(f, out, n_out, T, mode, bits, w_nwp, w_now, st);
+    if (c == 2) return linear_run<double, float>(f, out, n_out, T, mode, bits, w_nwp, w_now, st);
+    if (c == 3) return linear_run<double, double>(f, out, n_out, T, mode, bits, w_nwp, w_now, st);
+    b200::set_error("blend_linear: dtypes must be B200_F32 or B200_F64");
+    return B200_EINVAL;
+}
+
+extern "C" int b200_blend_salient(const void *now, int now_dtype, const int *now_map, int64_t now_member,
+                                  const void *nwp, int nwp_dtype, const int *nwp_map, int64_t nwp_member, void *out,
+                                  int n_out, int T, int64_t P, int lead, double w, double w1, double w2, double w12,
+                                  int fill_nwp, void *scratch, int64_t scratch_bytes, void *stream) {
+    const int64_t n = (int64_t)n_out * P;
+    B200_REQUIRE(n_out >= 0 && P >= 0 && n < ((int64_t)1 << 31) && lead >= 0 && lead < T, "bad arguments");
+    if (n == 0) return 0;
+    SortScratch s;
+    B200_REQUIRE(fields_ok(now, now_map, nwp, nwp_map, out) && scratch && scratch_bytes >= carve(&s, nullptr, n),
+                 "bad arguments");
+    const Fields f{now, now_map, now_member, nwp, nwp_map, nwp_member, P, fill_nwp};
+    cudaStream_t st = (cudaStream_t)stream;
+    const int c = now_dtype * 2 + nwp_dtype;
+    if (c == 0) return salient_run<float, float, float>(f, out, n_out, T, lead, w, w1, w2, w12, scratch, st);
+    if (c == 1) return salient_run<float, double, double>(f, out, n_out, T, lead, w, w1, w2, w12, scratch, st);
+    if (c == 2) return salient_run<double, float, double>(f, out, n_out, T, lead, w, w1, w2, w12, scratch, st);
+    if (c == 3) return salient_run<double, double, double>(f, out, n_out, T, lead, w, w1, w2, w12, scratch, st);
+    b200::set_error("blend_salient: dtypes must be B200_F32 or B200_F64");
+    return B200_EINVAL;
+}
+
+extern "C" int b200_dense_rank(const void *x, int dtype, int64_t n, unsigned *rank, unsigned *max_rank, int *nan_flag,
+                               void *scratch, int64_t scratch_bytes, void *stream) {
+    B200_REQUIRE(n >= 0 && n < ((int64_t)1 << 31), "bad arguments");
+    if (n == 0) return 0;
+    SortScratch s;
+    B200_REQUIRE(x && rank && max_rank && nan_flag && scratch && scratch_bytes >= carve(&s, nullptr, n),
+                 "bad arguments");
+    carve(&s, (char *)scratch, n);
+    cudaStream_t st = (cudaStream_t)stream;
+    B200_CUDA(cudaMemsetAsync(s.nan_flag, 0, 4, st));
+    if (dtype == B200_F32) array_keys<float><<<grid_for(n), THREADS, 0, st>>>((const float *)x, n, s.key[0], s.idx[0], s.nan_flag);
+    else if (dtype == B200_F64) array_keys<double><<<grid_for(n), THREADS, 0, st>>>((const double *)x, n, s.key[0], s.idx[0], s.nan_flag);
+    else {
+        b200::set_error("dense_rank: dtype must be B200_F32 or B200_F64");
+        return B200_EINVAL;
+    }
+    B200_LAUNCH_CHECK();
+    if (int rc = dense_rank(s, n, st)) return rc;
+    B200_CUDA(cudaMemcpyAsync(rank, s.rank, 4 * n, cudaMemcpyDeviceToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(max_rank, s.max_rank, 4, cudaMemcpyDeviceToDevice, st));
+    B200_CUDA(cudaMemcpyAsync(nan_flag, s.nan_flag, 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}

@@ -9,6 +9,10 @@ pysteps has no entry-point discovery for motion / extrapolation methods; the
                                               Lagrangian probability nowcast)
   pysteps/postprocessing/interface.py:29-33   ``_ensemblestats_methods`` ("mean", "excprob",
                                               "banddepth")
+  pysteps/blending/interface.py:20-24         ``_blending_methods`` ("linear_blending",
+                                              "salient_blending")
+The nowcasts "extrapolation" / "lagrangian" (the extrapolation nowcast) also go into
+``_nowcast_methods``.
 ``register()`` inserts the B200 callables under new names and, on request,
 under the stock names so that ``nowcasts.steps`` (which fetches the
 extrapolator by name at pysteps/nowcasts/steps.py:656 and
@@ -21,6 +25,8 @@ def methods():
     from .extrapolation import semilagrangian
 
     from .noise import motion as bps
+    from .blending import interface as blending
+    from .nowcasts import extrapolation as extrapolation_nowcast
     from .nowcasts import lagrangian_probability
     from .postprocessing import ensemblestats
 
@@ -29,7 +35,12 @@ def methods():
            "nowcasts": {"lagrangian_probability_b200": lagrangian_probability.forecast,
                         "probability_b200": lagrangian_probability.forecast},
            "ensemblestats": {"mean_b200": ensemblestats.mean, "excprob_b200": ensemblestats.excprob,
-                             "banddepth_b200": ensemblestats.banddepth}}
+                             "banddepth_b200": ensemblestats.banddepth},
+           # kept apart from "nowcasts" so that that entry still lists the probability models only
+           "extrapolation_nowcasts": {"extrapolation_b200": extrapolation_nowcast.forecast,
+                                      "lagrangian_b200": extrapolation_nowcast.forecast},
+           "blending": {"linear_blending_b200": blending.get_method("linear_blending"),
+                        "salient_blending_b200": blending.get_method("salient_blending")}}
     try:
         from .motion import lucaskanade
         out["motion"]["lk_b200"] = lucaskanade.dense_lucaskanade
@@ -57,8 +68,9 @@ def register(override=False):
     pysteps/tests/test_interfaces.py keep passing).  override=True additionally
     replaces ``"semilagrangian"``, ``"lk"``/``"lucaskanade"``, ``"vet"``, ``"proesmans"``,
     ``"constant"``, ``"darts"``, the noise method ``"bps"``, the nowcasts ``"probability"`` /
-    ``"lagrangian_probability"`` and the ensemble statistics ``"mean"``, ``"excprob"`` and
-    ``"banddepth"``.  Only the registries change: ``from pysteps.postprocessing.ensemblestats import
+    ``"lagrangian_probability"``, ``"extrapolation"`` / ``"lagrangian"``, the ensemble statistics
+    ``"mean"``, ``"excprob"`` and ``"banddepth"``, and the blending methods ``"linear_blending"`` and
+    ``"salient_blending"``.  Only the registries change: ``from pysteps.postprocessing.ensemblestats import
     excprob`` (and every other direct import) still gives the stock function.
     Returns the list of registered names.
     """
@@ -66,6 +78,7 @@ def register(override=False):
     import pysteps.motion.interface as mi
     import pysteps.noise.interface as ni
     import pysteps.nowcasts.interface as nci
+    import pysteps.blending.interface as bi
     import pysteps.postprocessing.interface as ppi
 
     done = []
@@ -88,7 +101,7 @@ def register(override=False):
         if override:
             ni._noise_methods[name.replace("_b200", "")] = fns
             done.append("noise:" + name.replace("_b200", ""))
-    for name, fn in m["nowcasts"].items():
+    for name, fn in list(m["nowcasts"].items()) + list(m["extrapolation_nowcasts"].items()):
         nci._nowcast_methods[name] = fn
         done.append("nowcasts:" + name)
         if override:
@@ -100,4 +113,10 @@ def register(override=False):
         if override:
             ppi._ensemblestats_methods[name.replace("_b200", "")] = fn
             done.append("ensemblestats:" + name.replace("_b200", ""))
+    for name, fn in m["blending"].items():
+        bi._blending_methods[name] = fn
+        done.append("blending:" + name)
+        if override:
+            bi._blending_methods[name.replace("_b200", "")] = fn
+            done.append("blending:" + name.replace("_b200", ""))
     return done

@@ -24,7 +24,7 @@ import torch
 from .. import _compare, _device, _lib
 from ..extrapolation import interface as _extrapolation
 from ..extrapolation import semilagrangian as _sl
-from ..noise import motion as _bps
+from . import extrapolation as _extrapolation_nowcast
 
 _MAX_SCALE = 1 << 24  # B200_PROBABILITY_MAX_SCALE
 
@@ -39,20 +39,7 @@ def forecast(precip, velocity, timesteps, threshold, extrap_method="semilagrangi
     elif not isinstance(timesteps, list):
         raise ValueError(f"invalid value for argument 'timesteps': {timesteps}")
 
-    # nowcasts/extrapolation.py:104-117
-    if precip.ndim != 2:
-        raise ValueError("The input precipitation must be a " "two-dimensional array")
-    if velocity.ndim != 3:
-        raise ValueError("Input velocity must be a three-dimensional array")
-    if precip.shape != velocity.shape[1:3]:
-        raise ValueError(
-            "Dimension mismatch between "
-            "input precipitation and velocity: "
-            + "shape(precip)=%s, shape(velocity)=%s"
-            % (str(precip.shape), str(velocity.shape))
-        )
-    if isinstance(timesteps, list) and not sorted(timesteps) == timesteps:
-        raise ValueError("timesteps is not in ascending order")
+    _extrapolation_nowcast.check_inputs(precip, velocity, timesteps)
 
     lib = torch if isinstance(precip, torch.Tensor) else np
     if precip.dtype not in (lib.float32, lib.float64):
@@ -72,10 +59,7 @@ def forecast(precip, velocity, timesteps, threshold, extrap_method="semilagrangi
 
     method = _extrapolation.get_method(extrap_method)
     if method is _sl.extrapolate:
-        vel = velocity
-        if not (_device.is_device_tensor(velocity) or isinstance(velocity, _bps.PerturbedVelocity)):
-            vel = _sl._field_tensor(velocity)
-        F = method(d_precip, vel, timesteps, **extrap_kwargs)
+        F = method(d_precip, _extrapolation_nowcast.device_velocity(velocity), timesteps, **extrap_kwargs)
     elif method is _extrapolation.eulerian_persistence and not extrap_kwargs.get("return_displacement", False):
         F = d_precip.unsqueeze(0).expand(len(timesteps), m, n)  # plane stride 0: the field is not replicated
     else:
