@@ -6,13 +6,13 @@ with saliency=True) are blending/linear_blending.py; "steps" and "pca_enkf" are 
 """
 from functools import partial
 
+from ..interface import with_b200_names
 from . import linear_blending
 
-_blending_methods = dict()
-_blending_methods["linear_blending"] = linear_blending.forecast
-_blending_methods["linear_blending_b200"] = linear_blending.forecast
-_blending_methods["salient_blending"] = partial(linear_blending.forecast, saliency=True)
-_blending_methods["salient_blending_b200"] = _blending_methods["salient_blending"]
+PROVIDED = {"linear_blending": linear_blending.forecast,
+            "salient_blending": partial(linear_blending.forecast, saliency=True)}
+
+_blending_methods = with_b200_names(PROVIDED)
 
 
 def get_method(name):

@@ -2,6 +2,7 @@
 semi-Lagrangian scheme behind the same ``get_method(name)`` contract."""
 import numpy as np
 
+from ..interface import with_b200_names
 from . import semilagrangian
 
 
@@ -25,10 +26,10 @@ def _do_nothing(precip, velocity, timesteps, outval=np.nan, **kwargs):
     return None
 
 
-_extrapolation_methods = dict()
+PROVIDED = {"semilagrangian": semilagrangian.extrapolate}
+
+_extrapolation_methods = with_b200_names(PROVIDED)
 _extrapolation_methods["eulerian"] = eulerian_persistence
-_extrapolation_methods["semilagrangian"] = semilagrangian.extrapolate
-_extrapolation_methods["semilagrangian_b200"] = semilagrangian.extrapolate
 _extrapolation_methods[None] = _do_nothing
 _extrapolation_methods["none"] = _do_nothing
 

@@ -8,35 +8,18 @@ farneback is not provided.
 """
 import numpy as np
 
+from ..interface import with_b200_names
+from .constant import constant
+from .darts import DARTS
 from .lucaskanade import dense_lucaskanade
+from .proesmans import proesmans
+from .vet import vet
 
-_methods = dict()
-_methods["lk"] = dense_lucaskanade
-_methods["lucaskanade"] = dense_lucaskanade
-_methods["lk_b200"] = dense_lucaskanade
+PROVIDED = {"lk": dense_lucaskanade, "lucaskanade": dense_lucaskanade, "vet": vet, "proesmans": proesmans,
+            "constant": constant, "darts": DARTS}
+
+_methods = with_b200_names(PROVIDED)
 _methods[None] = lambda precip, *args, **kw: np.zeros((2, precip.shape[1], precip.shape[2]))
-try:
-    from .vet import vet
-    _methods["vet"] = vet
-    _methods["vet_b200"] = vet
-except ImportError:  # VET not built yet
-    pass
-
-
-from .proesmans import proesmans  # noqa: E402
-
-_methods["proesmans"] = proesmans
-_methods["proesmans_b200"] = proesmans
-
-from .constant import constant  # noqa: E402
-
-_methods["constant"] = constant
-_methods["constant_b200"] = constant
-
-from .darts import DARTS  # noqa: E402
-
-_methods["darts"] = DARTS
-_methods["darts_b200"] = DARTS
 
 
 def get_method(name):

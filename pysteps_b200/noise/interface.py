@@ -2,11 +2,12 @@
 ``get_method("bps")`` -> (initialize_bps, generate_bps).  The precipitation noise generators
 (parametric, nonparametric, ssft, nested) are FFT filters outside this path and are not
 provided."""
+from ..interface import with_b200_names
 from . import motion
 
-_noise_methods = dict()
-_noise_methods["bps"] = (motion.initialize_bps, motion.generate_bps)
-_noise_methods["bps_b200"] = (motion.initialize_bps, motion.generate_bps)
+PROVIDED = {"bps": (motion.initialize_bps, motion.generate_bps)}
+
+_noise_methods = with_b200_names(PROVIDED)
 
 
 def get_method(name):

@@ -7,18 +7,14 @@ and "eulerian" the Eulerian persistence of extrapolation/interface.py; the other
 reference are not provided.
 """
 from ..extrapolation import interface as _extrapolation
+from ..interface import with_b200_names
 from . import extrapolation, lagrangian_probability
 
-_nowcast_methods = dict()
-_nowcast_methods["lagrangian_probability"] = lagrangian_probability.forecast
-_nowcast_methods["lagrangian_probability_b200"] = lagrangian_probability.forecast
-_nowcast_methods["probability"] = lagrangian_probability.forecast
-_nowcast_methods["probability_b200"] = lagrangian_probability.forecast
+PROVIDED = {"lagrangian_probability": lagrangian_probability.forecast, "probability": lagrangian_probability.forecast,
+            "extrapolation": extrapolation.forecast, "lagrangian": extrapolation.forecast}
+
+_nowcast_methods = with_b200_names(PROVIDED)
 _nowcast_methods["eulerian"] = _extrapolation.eulerian_persistence
-_nowcast_methods["extrapolation"] = extrapolation.forecast
-_nowcast_methods["extrapolation_b200"] = extrapolation.forecast
-_nowcast_methods["lagrangian"] = extrapolation.forecast
-_nowcast_methods["lagrangian_b200"] = extrapolation.forecast
 
 
 def get_method(name):

@@ -5,18 +5,14 @@ name or type that is not a string, ValueError for an unknown one.  The "ensemble
 postprocessing/ensemblestats.py under the reference's names and with a "_b200" suffix; there are no
 "diagnostics" methods, as in the reference without plugins.
 """
+from ..interface import with_b200_names
 from . import ensemblestats
+
+PROVIDED = {"mean": ensemblestats.mean, "excprob": ensemblestats.excprob, "banddepth": ensemblestats.banddepth}
 
 _diagnostics_methods = dict()
 
-_ensemblestats_methods = dict(
-    mean=ensemblestats.mean,
-    excprob=ensemblestats.excprob,
-    banddepth=ensemblestats.banddepth,
-    mean_b200=ensemblestats.mean,
-    excprob_b200=ensemblestats.excprob,
-    banddepth_b200=ensemblestats.banddepth,
-)
+_ensemblestats_methods = with_b200_names(PROVIDED)
 
 
 def get_method(name, method_type):

@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 import cpu_abi
+import registries
 from pysteps_b200 import _synthetic as syn
 
 
@@ -27,8 +28,9 @@ def ref():
     utils = importlib.import_module("pysteps.nowcasts.utils")
     noise = importlib.import_module("pysteps.noise.interface")
     import pysteps_b200
-    pysteps_b200.register()
-    return utils, noise
+    with registries.restored():
+        pysteps_b200.register()
+        yield utils, noise
 
 
 def _model(state, params):

@@ -12,6 +12,7 @@ import warnings
 import numpy as np
 import pytest
 import reference_cases as rc
+import registries
 
 pytestmark = pytest.mark.gpu
 
@@ -79,14 +80,12 @@ def test_steps_forecast_with_registered_b200_methods(ref):
     steps = ref.ref_module("pysteps.nowcasts.steps")
     ex_if = ref.ref_module("pysteps.extrapolation.interface")
     mo_if = ref.ref_module("pysteps.motion.interface")
-    no_if = ref.ref_module("pysteps.noise.interface")
     m = n = 200
     fr = syn.rain_frames(m, n, 3, 4, dx=2, dy=-1)
     R = np.where(fr > 0.1, 10 * np.log10(np.maximum(fr, 0.1)), -15.0)
     kw = dict(timesteps=4, n_ens_members=3, n_cascade_levels=4, precip_thr=-10.0, kmperpixel=1.0, timestep=5.0,
               noise_method="nonparametric", seed=42, num_workers=1)
-    saved = (dict(ex_if._extrapolation_methods), dict(mo_if._methods), dict(no_if._noise_methods))
-    try:
+    with registries.restored():
         V_stock = _quiet(mo_if.get_method("lk"), fr)
         want = _quiet(steps.forecast, R, V_stock, **kw)
         pysteps_b200.register(override=True)
@@ -95,10 +94,6 @@ def test_steps_forecast_with_registered_b200_methods(ref):
         assert np.abs(V - V_stock).max() <= 1e-12
         got = _quiet(steps.forecast, R, V_stock, **kw)
         got_resident = _quiet(steps.forecast, R, V_stock, extrap_kwargs={"b200_resident": True}, **kw)
-    finally:
-        for reg, old in zip((ex_if._extrapolation_methods, mo_if._methods, no_if._noise_methods), saved):
-            reg.clear()
-            reg.update(old)
     assert want.shape == got.shape == (3, 4, m, n) and np.isfinite(want).any()
     assert np.array_equal(want, got, equal_nan=True)
     assert np.array_equal(want, got_resident, equal_nan=True)
@@ -109,7 +104,6 @@ def test_nowcast_main_loop_ensemble_with_b200_methods(ref):
     from pysteps_b200 import _synthetic as syn
     utils = ref.ref_module("pysteps.nowcasts.utils")
     noise = ref.ref_module("pysteps.noise.interface")
-    pysteps_b200.register()
     m, n, members = 200, 240, 3
     precip = syn.rain_field(m, n, 5)
     velocity = 2.0 * syn.velocity_field(m, n, 5)
@@ -130,10 +124,12 @@ def test_nowcast_main_loop_ensemble_with_b200_methods(ref):
                                        extrap_kwargs=extrap_kwargs, velocity_pert_gen=perts, params=params,
                                        ensemble=True, num_ensemble_members=members)
 
-    for timesteps in (3, [0.5, 1.0, 2.25, 3.0]):
-        want = _quiet(run, "bps", "semilagrangian", {"allow_nonfinite_values": True}, timesteps)
-        got = _quiet(run, "bps_b200", "semilagrangian_b200", {"allow_nonfinite_values": True, "b200_resident": True},
-                     timesteps)
-        for g_member, w_member in zip(got, want):
-            for g, w in zip(g_member, w_member):
-                assert np.array_equal(g, w, equal_nan=True)
+    with registries.restored():
+        pysteps_b200.register()
+        for timesteps in (3, [0.5, 1.0, 2.25, 3.0]):
+            want = _quiet(run, "bps", "semilagrangian", {"allow_nonfinite_values": True}, timesteps)
+            got = _quiet(run, "bps_b200", "semilagrangian_b200",
+                         {"allow_nonfinite_values": True, "b200_resident": True}, timesteps)
+            for g_member, w_member in zip(got, want):
+                for g, w in zip(g_member, w_member):
+                    assert np.array_equal(g, w, equal_nan=True)
