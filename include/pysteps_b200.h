@@ -268,14 +268,23 @@ int b200_good_features(const float *eig, const uint8_t *valid, int m, int n, int
                        double quality_level, double min_distance, float *out_xy,
                        int *out_count, void *stream);
 
-/* Pyramid geometry of cv::buildOpticalFlowPyramid (HOST pointers, 8 entries each). */
+/* Pyramid levels the LK entry points hold: every level cv::buildOpticalFlowPyramid keeps for
+ * a frame below 2^32 pixels (a 16th halving needs both sides above 2^16). */
+#define B200_LK_MAX_LEVELS 16
+/* Pyramid geometry of cv::buildOpticalFlowPyramid (HOST pointers, B200_LK_MAX_LEVELS entries
+ * each).  max_level is not capped: a geometry deeper than B200_LK_MAX_LEVELS levels is refused
+ * with B200_EINVAL. */
 int b200_lk_pyramid_layout(int h, int w, int win_w, int win_h, int max_level, int *levels_out,
                            int64_t *offsets, int *hs, int *ws, int64_t *total_pixels);
 /* Gaussian pyramid (levels contiguous) and, if deriv != NULL, its Scharr pyramid. */
 int b200_lk_build_pyramid(const uint8_t *img, int h, int w, int win_w, int win_h, int max_level,
                           uint8_t *pyr, int16_t *deriv, void *stream);
 /* cv::calcOpticalFlowPyrLK (tracking/lucaskanade.py:171), flags = 0: next_pts (npts,2)
- * float32, status (npts) uint8; bit-identical to opencv-python 4.13.0. */
+ * float32, status (npts) uint8; bit-identical to opencv-python 4.13.0 for EVERY point, lost
+ * ones included (NaN coordinates fail the window bounds test as in its x86 build; NaN payloads
+ * are not part of the contract).  Windows of 1 .. 4096 pixels (cv2 itself wants both sides
+ * above 2); max_count and epsilon as cv::TermCriteria leaves them after calcOpticalFlowPyrLK's
+ * clamps (the caller applies them). */
 int b200_lk_track(const uint8_t *pyrI, const uint8_t *pyrJ, const int16_t *derivI, int h, int w,
                   int win_w, int win_h, int max_level, int max_count, double epsilon,
                   double min_eig_thr, const float *prev_pts, int npts, const int *npts_dev,

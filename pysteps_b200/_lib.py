@@ -17,6 +17,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "pysteps_b200.h")
 F32, F64 = 0, 1
 MODE_CONSTANT, MODE_NEAREST = 0, 1
 LAYOUT_PLANAR, LAYOUT_INTERLEAVED = 0, 1
+LK_MAX_LEVELS = 16  # B200_LK_MAX_LEVELS: entries of b200_lk_pyramid_layout's level arrays
 
 _lib = None
 _lock = threading.Lock()

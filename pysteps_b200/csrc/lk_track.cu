@@ -9,23 +9,24 @@
 // tail), which is what makes the 2500-pixel sums reproducible.
 //
 // Mapping: one CTA per feature, all pyramid levels inside the kernel (a feature's track is
-// independent of every other feature's).  The window (<= 64x64) lives in shared memory as
+// independent of every other feature's).  The window (<= 4096 pixels) lives in shared memory as
 // int16; patch extraction and the per-iteration mismatch products are data parallel over
 // the CTA; the ordered float32 accumulations are 15 (setup) / 10 (per iteration) independent
 // sequential chains run by the lanes of warp 0 out of shared memory.
+#include <climits>
+
 #include "common.cuh"
 
 namespace {
 
-constexpr int LK_MAX_LEVELS = 8;
 constexpr int LK_THREADS = 128;  // 9 CTAs/SM: 1000 features fit in one wave
 constexpr int W_BITS = 14;
 
 struct LKParams {
     const uint8_t *I, *J;   // pyramids (levels contiguous)
     const short2 *dI;       // Scharr derivative pyramid of I
-    size_t off[LK_MAX_LEVELS];
-    int h[LK_MAX_LEVELS], w[LK_MAX_LEVELS];
+    size_t off[B200_LK_MAX_LEVELS];
+    int h[B200_LK_MAX_LEVELS], w[B200_LK_MAX_LEVELS];
     int max_level;          // coarsest level index actually built
     int win_w, win_h, max_count;
     double eps2, min_eig_thr;
@@ -47,9 +48,17 @@ __device__ __forceinline__ int reflect101(int i, int L) {
 
 __device__ __forceinline__ int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
 
-// i / d for 0 <= i < 2^16 and 1 <= d <= 64 without an integer division (exact: the float
-// product is off by far less than the 0.5/d margin)
+// i / d for 0 <= i < 2^16 and any d >= 1 without an integer division (exact: (i + 0.5) / d sits
+// at least 0.5/d from an integer, and the two float roundings move it by at most
+// 2^-23 (i + 0.5) / d, which stays below that margin while i < 2^22)
 __device__ __forceinline__ int div_small(int i, float inv_d) { return __float2int_rd(((float)i + 0.5f) * inv_d); }
+
+// cvFloor as the x86 build of OpenCV computes it: NaN and values outside the int range give
+// INT_MIN (cvtss2si's "integer indefinite"), where cvt.rmi would give 0 for NaN and clamp the
+// rest.  Only the window bounds tests read it: a NaN coordinate must fail them as in cv2.
+__device__ __forceinline__ int cv_floor(float v) {
+    return (v >= -2147483648.f && v < 2147483648.f) ? __float2int_rd(v) : INT_MIN;
+}
 
 // bilinear fixed-point weights of a sub-pixel offset (a, b)
 __device__ __forceinline__ void make_weights(float a, float b, int &w00, int &w01, int &w10, int &w11) {
@@ -107,7 +116,7 @@ __global__ void __launch_bounds__(LK_THREADS) lk_track_kernel(const LKParams p) 
         else { nx = nx_out * 2.f; ny = ny_out * 2.f; }
         nx_out = nx; ny_out = ny;
         px -= half_x; py -= half_y;
-        const int ix = __float2int_rd(px), iy = __float2int_rd(py);
+        const int ix = cv_floor(px), iy = cv_floor(py);
         if (ix < -ww || ix >= w || iy < -wh || iy >= h) {
             if (level == 0) status = false;
             continue;
@@ -187,7 +196,7 @@ __global__ void __launch_bounds__(LK_THREADS) lk_track_kernel(const LKParams p) 
         nx -= half_x; ny -= half_y;
         float pdx = 0.f, pdy = 0.f;
         for (int j = 0; j < p.max_count; j++) {
-            const int jx = __float2int_rd(nx), jy = __float2int_rd(ny);
+            const int jx = cv_floor(nx), jy = cv_floor(ny);
             if (jx < -ww || jx >= w || jy < -wh || jy >= h) {
                 if (level == 0) status = false;
                 break;
@@ -264,7 +273,7 @@ __global__ void __launch_bounds__(LK_THREADS) lk_track_kernel(const LKParams p) 
         }
         if (status && level == 0) {
             // OpenCV's error pass re-checks that the final window origin is inside J
-            const int fx = __float2int_rd(nx_out - half_x), fy = __float2int_rd(ny_out - half_y);
+            const int fx = cv_floor(nx_out - half_x), fy = cv_floor(ny_out - half_y);
             if (fx < -ww || fx >= w || fy < -wh || fy >= h) status = false;
         }
     }
@@ -319,13 +328,13 @@ compact_tracks_kernel(const float *__restrict__ p0, const float *__restrict__ p1
 }  // namespace
 
 // Pyramid geometry of cv::buildOpticalFlowPyramid: level sizes (h+1)/2, a level is kept only
-// while both dimensions exceed the window.  Returns the coarsest level index and the total
-// number of pixels of all levels (levels are stored contiguously).
+// while both dimensions exceed the window, and max_level is not capped.  Returns the coarsest
+// level index and the total number of pixels of all levels (levels are stored contiguously).
+// B200_LK_MAX_LEVELS levels hold every geometry: a 16th halving needs both sides above 2^16.
 extern "C" int b200_lk_pyramid_layout(int h, int w, int win_w, int win_h, int max_level,
-                                      int *levels_out, int64_t *offsets /*[8]*/, int *hs, int *ws,
+                                      int *levels_out, int64_t *offsets, int *hs, int *ws,
                                       int64_t *total_pixels) {
     B200_REQUIRE(h >= 1 && w >= 1 && win_w >= 1 && win_h >= 1 && max_level >= 0, "bad arguments");
-    if (max_level > LK_MAX_LEVELS - 1) max_level = LK_MAX_LEVELS - 1;
     int lv = 0;
     int64_t off = 0;
     int ch = h, cw = w;
@@ -338,6 +347,7 @@ extern "C" int b200_lk_pyramid_layout(int h, int w, int win_w, int win_h, int ma
         if (level == max_level) break;
         const int nh = (ch + 1) / 2, nw = (cw + 1) / 2;
         if (nw <= win_w || nh <= win_h) break;
+        B200_REQUIRE(level + 1 < B200_LK_MAX_LEVELS, "pyramid deeper than B200_LK_MAX_LEVELS levels");
         ch = nh; cw = nw;
     }
     if (levels_out) *levels_out = lv;
@@ -354,8 +364,8 @@ extern "C" int b200_lk_build_pyramid(const uint8_t *img, int h, int w, int win_w
                                      int max_level, uint8_t *pyr, int16_t *deriv, void *stream) {
     // img == NULL: the Gaussian levels in `pyr` already exist, only derivatives are computed
     B200_REQUIRE(pyr && (img || deriv), "bad arguments");
-    int lv, hs[LK_MAX_LEVELS], ws[LK_MAX_LEVELS];
-    int64_t off[LK_MAX_LEVELS], total;
+    int lv, hs[B200_LK_MAX_LEVELS], ws[B200_LK_MAX_LEVELS];
+    int64_t off[B200_LK_MAX_LEVELS], total;
     int rc = b200_lk_pyramid_layout(h, w, win_w, win_h, max_level, &lv, off, hs, ws, &total);
     if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
@@ -384,7 +394,7 @@ extern "C" int b200_lk_track(const uint8_t *pyrI, const uint8_t *pyrJ, const int
     LKParams p;
     memset(&p, 0, sizeof(p));
     int lv;
-    int64_t off[LK_MAX_LEVELS], total;
+    int64_t off[B200_LK_MAX_LEVELS], total;
     int rc = b200_lk_pyramid_layout(h, w, win_w, win_h, max_level, &lv, off, p.h, p.w, &total);
     if (rc) return rc;
     for (int l = 0; l <= lv; l++) p.off[l] = (size_t)off[l];

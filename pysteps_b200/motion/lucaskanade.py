@@ -150,13 +150,34 @@ def _side_stream():
 
 def _pyramid_layout(m, n, win, max_level):
     lv = ctypes.c_int(0)
-    off = (ctypes.c_int64 * 8)()
-    hs = (ctypes.c_int * 8)()
-    ws = (ctypes.c_int * 8)()
+    off = (ctypes.c_int64 * _lib.LK_MAX_LEVELS)()
+    hs = (ctypes.c_int * _lib.LK_MAX_LEVELS)()
+    ws = (ctypes.c_int * _lib.LK_MAX_LEVELS)()
     tot = ctypes.c_int64(0)
     _lib.check(_lib.load().b200_lk_pyramid_layout(m, n, int(win[0]), int(win[1]), int(max_level),
                                                   ctypes.byref(lv), off, hs, ws, ctypes.byref(tot)))
     return lv.value, int(tot.value)
+
+
+_WINDOW_MAX = 64 * 64  # csrc/lk_track.cu: the window and its products live in one CTA's shared memory
+
+
+def _tracker_args(winsize, nr_levels, criteria):
+    """calcOpticalFlowPyrLK's argument check and TermCriteria clamps (tracking/lucaskanade.py:171), taken
+    before anything is uploaded -> (win_w, win_h, nr_levels, max_count, epsilon).  cv2 raises its
+    assertion as cv2.error, even without points to track; here it is a ValueError with the same text."""
+    win_w, win_h = (int(v) for v in winsize)
+    nr_levels = int(nr_levels)
+    if not (nr_levels >= 0 and win_w > 2 and win_h > 2):
+        raise ValueError("(-215:Assertion failed) maxLevel >= 0 && winSize.width > 2 && winSize.height > 2 "
+                         "in function 'calc'")
+    if win_w * win_h > _WINDOW_MAX:
+        raise NotImplementedError(f"pysteps_b200 LK: tracking windows above {_WINDOW_MAX} pixels are not "
+                                  f"implemented (winsize {win_w}x{win_h})")
+    ctype, max_count, eps = criteria
+    max_count = min(max(int(max_count), 0), 100) if (int(ctype) & 1) else 30
+    eps = min(max(float(eps), 0.0), 10.0) if (int(ctype) & 2) else 0.01
+    return win_w, win_h, nr_levels, max_count, eps
 
 
 _KD_SHARED_MAX = 4096  # csrc/knn_device.cuh NMAX: the tree of the tie recomputation is built in one CTA
@@ -314,15 +335,12 @@ def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kw
         raise NotImplementedError("pysteps_b200 LK: max_corners must be positive")
     max_corners = int(max_corners)
     # tracking.lucaskanade.track_features defaults (tracking/lucaskanade.py:35-45)
-    winsize = tuple(lk_kwargs.get("winsize", (50, 50)))
-    nr_levels = int(lk_kwargs.get("nr_levels", 3))
-    criteria = tuple(lk_kwargs.get("criteria", (3, 10, 0)))
     if lk_kwargs.get("flags", 0) != 0:
         raise NotImplementedError("pysteps_b200 LK: flags must be 0")
+    win_w, win_h, nr_levels, max_count, eps = _tracker_args(lk_kwargs.get("winsize", (50, 50)),
+                                                            lk_kwargs.get("nr_levels", 3),
+                                                            tuple(lk_kwargs.get("criteria", (3, 10, 0))))
     min_eig_thr = float(lk_kwargs.get("min_eig_thr", 1e-4))
-    ctype, max_count, eps = criteria
-    max_count = min(max(int(max_count), 0), 100) if (int(ctype) & 1) else 30
-    eps = min(max(float(eps), 0.0), 10.0) if (int(ctype) & 2) else 0.01
 
     nr_fields = int(input_images.shape[0])
     m, n = int(input_images.shape[1]), int(input_images.shape[2])
@@ -382,7 +400,7 @@ def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kw
     pool_xy = torch.empty((pool_cap, 2), dtype=torch.float64, device="cuda")
     pool_uv = torch.empty((pool_cap, 2), dtype=torch.float64, device="cuda")
     counts = torch.zeros(4, dtype=torch.int32, device="cuda")  # pool, kept, declustered, corners
-    lv, total = _pyramid_layout(m, n, winsize, nr_levels)
+    lv, total = _pyramid_layout(m, n, (win_w, win_h), nr_levels)
     # pyramids: Gaussian levels of every frame, Scharr levels of every frame but the last
     pyr = [[torch.empty(total, dtype=torch.uint8, device="cuda"),
             torch.empty(2 * total, dtype=torch.int16, device="cuda") if t < nr_fields - 1 else None,
@@ -391,7 +409,7 @@ def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kw
     def pyramid(t, with_deriv):
         """Gaussian pyramid of frame t's uint8 image (+ Scharr pyramid when it is the previous
         frame of a pair); a middle frame is built once and reused by both of its pairs."""
-        args = (m, n, int(winsize[0]), int(winsize[1]), nr_levels)
+        args = (m, n, win_w, win_h, nr_levels)
         P, D, have_p, have_d = pyr[t]
         want_d = with_deriv and not have_d
         if not have_p:
@@ -439,7 +457,7 @@ def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kw
         nxt = torch.empty((max_corners, 2), dtype=torch.float32, device="cuda")
         status = torch.empty(max_corners, dtype=torch.uint8, device="cuda")
         _call("b200_lk_track", pI[0].data_ptr(), pJ[0].data_ptr(), pI[1].data_ptr(), m, n,
-              int(winsize[0]), int(winsize[1]), nr_levels, max_count, eps, min_eig_thr,
+              win_w, win_h, nr_levels, max_count, eps, min_eig_thr,
               corners.data_ptr(), max_corners, ncorner.data_ptr(), nxt.data_ptr(), status.data_ptr(),
               _s())
         _call("b200_lk_compact_tracks", corners.data_ptr(), nxt.data_ptr(), status.data_ptr(),

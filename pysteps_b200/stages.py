@@ -101,14 +101,12 @@ def track_features(prvs_image, next_image, points, winsize=(50, 50), nr_levels=3
     if flags != 0:
         raise NotImplementedError("pysteps_b200 track_features: flags must be 0")
     m, n = prvs_image.shape
-    ctype, max_count, eps = criteria
-    max_count = min(max(int(max_count), 0), 100) if (int(ctype) & 1) else 30
-    eps = min(max(float(eps), 0.0), 10.0) if (int(ctype) & 2) else 0.01
+    win_w, win_h, nr_levels, max_count, eps = _lk._tracker_args(winsize, nr_levels, criteria)
     p0 = np.ascontiguousarray(points, dtype=np.float32).reshape(-1, 2)
     npts = p0.shape[0]
     if npts == 0:
         return np.empty(shape=(0, 2)), np.empty(shape=(0, 2))
-    lv, total = _lk._pyramid_layout(m, n, winsize, nr_levels)
+    lv, total = _lk._pyramid_layout(m, n, (win_w, win_h), nr_levels)
     pyrs = []
     for image, deriv in ((prvs_image, True), (next_image, False)):
         img, um = _frame(image)
@@ -117,14 +115,14 @@ def track_features(prvs_image, next_image, points, winsize=(50, 50), nr_levels=3
         q = _lk._track_image(f, m, n, 0)
         P = torch.empty(total, dtype=torch.uint8, device="cuda")
         D = torch.empty(2 * total, dtype=torch.int16, device="cuda") if deriv else None
-        _lib.call("b200_lk_build_pyramid", q.data_ptr(), m, n, int(winsize[0]), int(winsize[1]),
-                  int(nr_levels), P.data_ptr(), _device.ptr(D), _s())
+        _lib.call("b200_lk_build_pyramid", q.data_ptr(), m, n, win_w, win_h, nr_levels, P.data_ptr(),
+                  _device.ptr(D), _s())
         pyrs.append((P, D, f))
     d0 = _device.to_device(p0)
     d1 = torch.empty((npts, 2), dtype=torch.float32, device="cuda")
     st = torch.empty(npts, dtype=torch.uint8, device="cuda")
     _lib.call("b200_lk_track", pyrs[0][0].data_ptr(), pyrs[1][0].data_ptr(), pyrs[0][1].data_ptr(), m, n,
-              int(winsize[0]), int(winsize[1]), int(nr_levels), max_count, eps, float(min_eig_thr),
+              win_w, win_h, nr_levels, max_count, eps, float(min_eig_thr),
               d0.data_ptr(), npts, None, d1.data_ptr(), st.data_ptr(), _s())
     p1 = d1.cpu().numpy()
     keep = st.cpu().numpy() == 1

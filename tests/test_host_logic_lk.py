@@ -230,3 +230,82 @@ def test_many_frames_pool_larger_than_the_decluster_kernel(monkeypatch):
         monkeypatch.setattr(lkmod, "_DECLUSTER_MAX", 3)
         with pytest.raises(NotImplementedError, match="declustering more than 3"):
             lkmod.dense_lucaskanade(fr)
+
+
+@pytest.mark.parametrize("lk_kwargs,error,match", [
+    (dict(winsize=(2, 2)), ValueError, "winSize.width > 2 && winSize.height > 2"),
+    (dict(winsize=(3, 2)), ValueError, "winSize.width > 2 && winSize.height > 2"),
+    (dict(winsize=(1, 5000)), ValueError, "winSize.width > 2 && winSize.height > 2"),
+    (dict(nr_levels=-1), ValueError, "maxLevel >= 0"),
+    (dict(winsize=(65, 65)), NotImplementedError, "tracking windows above 4096 pixels"),
+    (dict(winsize=(4097, 3)), NotImplementedError, "tracking windows above 4096 pixels"),
+])
+def test_tracker_arguments_are_refused_before_anything_is_uploaded(lk_kwargs, error, match):
+    """Windows with a side below 3 and negative level counts fail cv2's assertion (a ValueError with its
+    text here: cv2.error cannot be imported without cv2); windows above 4096 pixels, which the device
+    does not hold, raise NotImplementedError.  Both before any upload or launch, in dense_lucaskanade and
+    in stages.track_features -- even without points to track, as cv2 asserts first."""
+    from unittest import mock
+
+    import torch
+    from pysteps_b200 import _device, _lib, stages
+    from pysteps_b200.motion.lucaskanade import dense_lucaskanade
+
+    def refuse(*a, **k):
+        raise AssertionError("device work before the tracker arguments were checked")
+
+    fr = syn.rain_frames(96, 112, 2, 3, dx=2, dy=-1)
+    kw = dict(dict(winsize=(50, 50), nr_levels=3), **lk_kwargs)
+    with cpu_abi.emulated(), mock.patch.object(_lib, "call", refuse), \
+            mock.patch.object(_device, "to_device", refuse), mock.patch.object(torch, "empty", refuse):
+        with pytest.raises(error, match=match):
+            dense_lucaskanade(fr, lk_kwargs=lk_kwargs)
+        with pytest.raises(error, match=match):
+            stages.track_features(fr[0], fr[1], np.float32([[40.0, 30.0]]), **kw)
+        with pytest.raises(error, match=match):
+            stages.track_features(fr[0], fr[1], np.empty((0, 2), np.float32), **kw)
+    live = _live()
+    if live is not None and error is ValueError:
+        import cv2
+        with pytest.raises(cv2.error) as e:
+            live(fr.copy(), lk_kwargs=lk_kwargs)
+        with pytest.raises(ValueError) as ours, cpu_abi.emulated():
+            dense_lucaskanade(fr.copy(), lk_kwargs=lk_kwargs)
+        assert str(ours.value) in str(e.value)
+
+
+def test_tracker_criteria_are_clamped_like_cv2():
+    """TermCriteria as calcOpticalFlowPyrLK leaves it: COUNT clamps max_count to 0 .. 100 (30 without
+    it), EPS clamps epsilon to 0 .. 10 (0.01 without it)."""
+    from pysteps_b200.motion.lucaskanade import _tracker_args
+    for crit, want in (((3, 10, 0), (10, 0.0)), ((1, 10, 0.5), (10, 0.01)), ((2, 10, 0.5), (30, 0.5)),
+                       ((3, 500, 20.0), (100, 10.0)), ((3, -5, -1.0), (0, 0.0)), ((0, 7, 7.0), (30, 0.01))):
+        assert _tracker_args((21, 21), 3, crit)[3:] == want, crit
+    assert _tracker_args((63, 65), 0, (3, 10, 0))[:3] == (63, 65, 0)
+    assert _tracker_args((64, 64), 20, (3, 10, 0))[:3] == (64, 64, 20)
+
+
+@pytest.mark.parametrize("shape,win,levels", [
+    ((300, 340), (50, 50), 3), ((300, 340), (7, 7), 9), ((20, 26), (21, 21), 3), ((1, 1), (3, 3), 4),
+    ((1024, 1024), (3, 3), 7), ((1024, 1024), (3, 3), 8), ((1024, 1024), (3, 3), 10), ((2048, 2048), (3, 3), 30),
+    ((46340, 46340), (1, 1), 40), ((65537, 65537), (1, 1), 15), ((3, 70000), (1, 1), 40), ((513, 1025), (3, 3), 0)])
+def test_pyramid_layout_keeps_every_level_cv2_builds(shape, win, levels):
+    """b200_lk_pyramid_layout (host code of the library) against cv::buildOpticalFlowPyramid's rule, with no
+    cap on the level count: nine levels at 1024^2 with a 3x3 window, sixteen for the deepest geometry of a
+    frame below 2^32 pixels."""
+    from pysteps_b200.motion.lucaskanade import _pyramid_layout
+    from lk_track_edges import pyramid_sizes
+    sizes = pyramid_sizes(shape[0], shape[1], win, levels)
+    lv, total = _pyramid_layout(shape[0], shape[1], win, levels)
+    assert (lv, total) == (len(sizes) - 1, sum(h * w for h, w in sizes))
+
+
+def test_pyramid_layout_refuses_a_pyramid_deeper_than_its_arrays():
+    from pysteps_b200 import _lib
+    from pysteps_b200.motion.lucaskanade import _pyramid_layout
+    from lk_track_edges import pyramid_sizes
+    assert len(pyramid_sizes(65537, 65537, (1, 1), 40)) == _lib.LK_MAX_LEVELS + 1
+    with pytest.raises(RuntimeError, match="deeper than B200_LK_MAX_LEVELS"):
+        _pyramid_layout(65537, 65537, (1, 1), 40)
+    with open(_lib.HEADER_PATH) as f:
+        assert f"#define B200_LK_MAX_LEVELS {_lib.LK_MAX_LEVELS}\n" in f.read()
