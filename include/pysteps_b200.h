@@ -613,6 +613,57 @@ int b200_blend_salient(const void *now, int now_dtype, const int *now_map, int64
 int b200_dense_rank(const void *x, int dtype, int64_t n, unsigned *rank, unsigned *max_rank, int *nan_flag,
                     void *scratch, int64_t scratch_bytes, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Verification scores (pysteps/verification/probscores.py, ensscores.py): the accumulation steps of
+ * CRPS, the rank histogram, the reliability diagram and the ROC curve.  X_f is a (k, N) ensemble
+ * (member i at X_f + i * N elements), X_o, P the (N) observations and probabilities, each of dtype
+ * B200_F32 or B200_F64; N < 2^31.  Thresholds are doubles already rounded to NumPy's comparison
+ * dtype and compared in double.  Device memory unless stated otherwise. */
+#define B200_VERIF_MAX_MEMBERS 512 /* k of b200_verif_crps and b200_verif_rankhist */
+#define B200_VERIF_MAX_BINS 2048   /* n_bins of b200_verif_reldiag, n_thr of b200_verif_roc */
+
+/* out[s] (nseg values of `dtype`) = np.sum(x[seg_off[s] : seg_off[s] + seg_len[s]]): NumPy's pairwise
+ * summation in `dtype` (csrc/pairwise_body.cuh).  seg_off, seg_len: HOST arrays.  Only enqueues
+ * kernels. */
+int b200_pairwise_sum(const void *x, int dtype, const int64_t *seg_off, const int64_t *seg_len, int nseg,
+                      void *out, void *stream);
+
+/* CRPS: at every pixel whose members and observation are finite, in pixel order, res[j] = the
+ * pixel's np.sum over its k + 1 columns of alpha p^2 + beta (1 - p)^2 (float64); *n (device int64)
+ * the number of such pixels.  res: N doubles.  1 <= k <= B200_VERIF_MAX_MEMBERS.  Only enqueues
+ * kernels. */
+int b200_verif_crps(const void *Xf, int f_dtype, const void *Xo, int o_dtype, int k, int64_t N, double *res,
+                    int64_t *n, void *stream);
+
+/* Rank histogram, step 1.  The pixels whose members and observation are finite (and, with use_min,
+ * some member >= thr_f or the observation >= thr_o); with use_min the values below their threshold
+ * become sub_f / sub_o (already in the array's dtype).  b1 = #{members < obs}, b2 = k - #{members >
+ * obs}.  hist (k + 1 int64, zeroed by the call) counts every untied pixel in bin b1; ties (N int32
+ * pairs) receive (b1, b2) of the tied pixels in pixel order and *n_ties (device int64) their number.
+ * 1 <= k <= B200_VERIF_MAX_MEMBERS.  Only enqueues kernels. */
+int b200_verif_rankhist(const void *Xf, int f_dtype, const void *Xo, int o_dtype, int k, int64_t N, int use_min,
+                        double thr_f, double sub_f, double thr_o, double sub_o, int64_t *hist, void *ties,
+                        int64_t *n_ties, void *stream);
+
+/* Rank histogram, step 2: hist[int(b1 + u[j] * (b2 + 1 - b1))] += 1 for the n_ties tied pixels of
+ * step 1, u (n_ties float64) the uniform draws.  Only enqueues kernels. */
+int b200_verif_rankhist_ties(const void *ties, int64_t n_ties, const double *u, int k, int64_t *hist,
+                             void *stream);
+
+/* Reliability diagram: the finite pairs, binned by np.digitize(P, edges, right=True) over the
+ * n_edges increasing float64 edges (HOST array), n_edges - 1 <= B200_VERIF_MAX_BINS.  For the bins
+ * 1 .. n_edges - 1: above[bin - 1] (int64) = #{obs >= thr_o}; sorted (N values of p_dtype) = P of
+ * those pixels ordered by bin, in pixel order within a bin; seg (n_edges int64) = where every bin
+ * starts in sorted, then their total.  Only enqueues kernels. */
+int b200_verif_reldiag(const void *P, int p_dtype, const void *Xo, int o_dtype, int64_t N, const double *edges,
+                       int n_edges, double thr_o, void *sorted, int64_t *seg, int64_t *above, void *stream);
+
+/* ROC curve: counts (2 (n_thr + 1) int64): counts[c] the finite pairs with obs >= thr_o and exactly c
+ * of the n_thr increasing float64 thresholds (HOST array) <= P, counts[n_thr + 1 + c] those with obs <
+ * thr_o.  n_thr <= B200_VERIF_MAX_BINS.  Only enqueues kernels. */
+int b200_verif_roc(const void *P, int p_dtype, const void *Xo, int o_dtype, int64_t N, const double *thr, int n_thr,
+                   double thr_o, int64_t *counts, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -18,6 +18,7 @@ F32, F64 = 0, 1
 MODE_CONSTANT, MODE_NEAREST = 0, 1
 LAYOUT_PLANAR, LAYOUT_INTERLEAVED = 0, 1
 LK_MAX_LEVELS = 16  # B200_LK_MAX_LEVELS: entries of b200_lk_pyramid_layout's level arrays
+VERIF_MAX_MEMBERS, VERIF_MAX_BINS = 512, 2048  # B200_VERIF_MAX_MEMBERS / _MAX_BINS
 
 _lib = None
 _lock = threading.Lock()
@@ -140,6 +141,15 @@ _SIGNATURES = {
                                    c_int, c_int, c_i64, c_int, c_double, c_double, c_double, c_double, c_int,
                                    c_void_p, c_i64, c_void_p]),
     "b200_dense_rank": (c_int, [c_void_p, c_int, c_i64, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p]),
+    "b200_pairwise_sum": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "b200_verif_crps": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_i64, c_void_p, c_void_p, c_void_p]),
+    "b200_verif_rankhist": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_i64, c_int, c_double, c_double,
+                                    c_double, c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_verif_rankhist_ties": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_void_p, c_void_p]),
+    "b200_verif_reldiag": (c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_dp, c_int, c_double, c_void_p,
+                                   c_void_p, c_void_p, c_void_p]),
+    "b200_verif_roc": (c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_dp, c_int, c_double, c_void_p,
+                               c_void_p]),
 }
 
 
