@@ -664,6 +664,66 @@ int b200_verif_reldiag(const void *P, int p_dtype, const void *Xo, int o_dtype, 
 int b200_verif_roc(const void *P, int p_dtype, const void *Xo, int o_dtype, int64_t N, const double *thr, int n_thr,
                    double thr_o, int64_t *counts, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Deterministic and spatial verification scores (pysteps/verification/detcatscores.py,
+ * spatialscores.py, ensscores.py). */
+
+/* Contingency table of det_cat_fct_accum: pred and obs are C-contiguous arrays of the same shape,
+ * read at offset(kept index) + offset(reduced index), where each set of axes (at most 4, sizes and
+ * element strides in HOST arrays, slowest first; none: one element) is walked in C order.  For every
+ * output element m (M = the product of the kept sizes): counts[m], counts[M + m], counts[2M + m],
+ * counts[3M + m] (int64) = the hits (pred > thr_p and obs > thr_o), false alarms, misses and correct
+ * negatives over its reduced pairs.  NaN compares false.  M * R < 2^31.  Only enqueues kernels. */
+int b200_verif_contab(const void *pred, int p_dtype, const void *obs, int o_dtype, double thr_p, double thr_o,
+                      const int64_t *kept_size, const int64_t *kept_stride, int n_kept, const int64_t *red_size,
+                      const int64_t *red_stride, int n_red, int64_t *counts, void *stream);
+
+/* Moments of det_cont_fct_accum.  pred, obs: C-contiguous arrays of the same shape; NumPy's reduction
+ * order as a plan: for every output element m (M = the product of the kept sizes) and every outer
+ * index o (O = the product of the outer sizes, C order), a run of L contiguous elements starts at
+ * offset(m) + offset(o) (axes as for b200_verif_contab).  conditioning: 0 every pair, 1 the pairs with
+ * pred > thr_p or obs > thr_o, 2 both (the others become NaN).  For the nine summands k of the
+ * reference's np.nanmean calls (0 obs, 1 pred, 2 res = pred - obs, 3 res^2, 4 (pred + obs)^2,
+ * 5 |res|, 6 (obs - mobs)(pred - mpred), 7 |obs - mobs|^2, 8 |pred - mpred|^2, with the means mobs,
+ * mpred of 0 and 1 broadcast): tot[k M + m] (double) = NumPy's np.sum of the summand with NaN as 0 in
+ * its dtype (obs: obs's, pred: pred's, res-based: the result type); cnt[m] (int64) = the finite
+ * residuals and cnt[(1 + k) M + m] the non-NaN summands; infs[m] bit 2k / 2k + 1: +inf / -inf was
+ * summed; *flags the B200_MOM_* bits of the element-wise operations.  M O L < 2^31.  Only enqueues
+ * kernels. */
+#define B200_MOM_SUB_RES_OVER (1 << 0) /* pred - obs overflowed */
+#define B200_MOM_SUB_RES_INV (1 << 1)  /* pred - obs made a NaN from non-NaN operands */
+#define B200_MOM_ADD_SUM_OVER (1 << 2)
+#define B200_MOM_ADD_SUM_INV (1 << 3)
+#define B200_MOM_SQ_RES_OVER (1 << 4)
+#define B200_MOM_SQ_SUM_OVER (1 << 5)
+#define B200_MOM_SUB_OBS_OVER (1 << 6) /* obs - mobs */
+#define B200_MOM_SUB_OBS_INV (1 << 7)
+#define B200_MOM_SUB_PRED_OVER (1 << 8)
+#define B200_MOM_SUB_PRED_INV (1 << 9)
+#define B200_MOM_MUL_OVER (1 << 10) /* (obs - mobs) * (pred - mpred) */
+#define B200_MOM_MUL_INV (1 << 11)
+#define B200_MOM_SQ_VOBS_OVER (1 << 12)
+#define B200_MOM_SQ_VPRED_OVER (1 << 13)
+int b200_verif_cont_moments(const void *pred, int p_dtype, const void *obs, int o_dtype, int conditioning,
+                            double thr_p, double thr_o, const int64_t *kept_size, const int64_t *kept_stride,
+                            int n_kept, const int64_t *outer_size, const int64_t *outer_stride, int n_outer,
+                            int64_t L, double *tot, int64_t *cnt, int *infs, int *flags, void *stream);
+
+#define B200_FSS_GROUP 16 /* na, nb of b200_fss_sums */
+
+/* Fractions of fss_accum for nf fields of m x n values of `dtype` (field f at X + f m n): the
+ * indicator (x >= thr, a non-finite x taken as sub, both already rounded as NumPy rounds them),
+ * smoothed with scipy.ndimage.uniform_filter(size=s, mode="constant") when s > 1, into S (nf m n
+ * float64).  nf m n < 2^31.  Only enqueues kernels. */
+int b200_fss_fractions(const void *X, int dtype, int nf, int m, int n, double thr, double sub, int s, double *S,
+                       void *stream);
+
+/* out[i nb + j] = np.sum(S[a0 + i] * S[b0 + j]) over the P values of each plane (NumPy's pairwise
+ * summation, float64) for every i < na, j < nb with a0 + i <= b0 + j; the other entries are left as
+ * they are.  S: planes of P float64, plane f at S + f P.  na, nb <= B200_FSS_GROUP, P < 2^31.  Only
+ * enqueues kernels. */
+int b200_fss_sums(const double *S, int64_t P, int a0, int na, int b0, int nb, double *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,11 @@ MODE_CONSTANT, MODE_NEAREST = 0, 1
 LAYOUT_PLANAR, LAYOUT_INTERLEAVED = 0, 1
 LK_MAX_LEVELS = 16  # B200_LK_MAX_LEVELS: entries of b200_lk_pyramid_layout's level arrays
 VERIF_MAX_MEMBERS, VERIF_MAX_BINS = 512, 2048  # B200_VERIF_MAX_MEMBERS / _MAX_BINS
+FSS_GROUP = 16  # B200_FSS_GROUP: fields per group of b200_fss_sums
+# B200_MOM_*: the element-wise operations of b200_verif_cont_moments that overflowed (OVER) or made a NaN (INV)
+(MOM_SUB_RES_OVER, MOM_SUB_RES_INV, MOM_ADD_SUM_OVER, MOM_ADD_SUM_INV, MOM_SQ_RES_OVER, MOM_SQ_SUM_OVER,
+ MOM_SUB_OBS_OVER, MOM_SUB_OBS_INV, MOM_SUB_PRED_OVER, MOM_SUB_PRED_INV, MOM_MUL_OVER, MOM_MUL_INV, MOM_SQ_VOBS_OVER,
+ MOM_SQ_VPRED_OVER) = (1 << i for i in range(14))
 
 _lib = None
 _lock = threading.Lock()
@@ -150,6 +155,16 @@ _SIGNATURES = {
                                    c_void_p, c_void_p, c_void_p]),
     "b200_verif_roc": (c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_dp, c_int, c_double, c_void_p,
                                c_void_p]),
+    "b200_verif_contab": (c_int, [c_void_p, c_int, c_void_p, c_int, c_double, c_double, ctypes.POINTER(c_i64),
+                                  ctypes.POINTER(c_i64), c_int, ctypes.POINTER(c_i64), ctypes.POINTER(c_i64), c_int,
+                                  c_void_p, c_void_p]),
+    "b200_verif_cont_moments": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_double, c_double,
+                                        ctypes.POINTER(c_i64), ctypes.POINTER(c_i64), c_int, ctypes.POINTER(c_i64),
+                                        ctypes.POINTER(c_i64), c_int, c_i64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p]),
+    "b200_fss_fractions": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_int, c_void_p,
+                                   c_void_p]),
+    "b200_fss_sums": (c_int, [c_void_p, c_i64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
 }
 
 
