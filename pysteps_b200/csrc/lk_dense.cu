@@ -106,11 +106,14 @@ morph_open_kernel(const double *__restrict__ img, const uint8_t *__restrict__ ma
     out[i] = o;
 }
 
-// min/max/count over unmasked pixels of all rows (set 0), of rows >= 1 (set 1) and of rows >= 2
-// (set 2), plus (set 3, count only) the number of pixels whose k x k dilated mask is clear.
+// min/max/count over unmasked pixels of all rows (set 0), of the rows left when the detector masks
+// row 0 alone or row 1 alone (set 1) and of rows >= 2 (set 2), plus (set 3, count only) the number
+// of pixels whose k x k dilated mask is clear.
 // The row sets exist because feature/shitomasi.py:139 indexes the image with the uint8 mask
 // (`input_image[mask] = masked`): NumPy treats it as INTEGER indexing, which masks row 0 when
 // the buffered mask contains a 0 and row 1 when it contains a 1 -- not the buffered pixels.
+// Nothing masked: the buffered mask is all 0, row 0 goes and set 1 is rows >= 1.  Something masked:
+// set 1 serves only the case where the buffered mask is all 1 and row 1 alone goes -- rows != 1.
 __global__ void __launch_bounds__(TX *TY)
 masked_minmax_kernel(const double *__restrict__ img, const uint8_t *__restrict__ mask, int m, int n,
                      int dil, const double *__restrict__ stats0, MM *__restrict__ part, int nparts) {
@@ -129,7 +132,7 @@ masked_minmax_kernel(const double *__restrict__ img, const uint8_t *__restrict__
         bool d = mask[i] != 0;
         if (!d) {
             a[0].mn = fmin(a[0].mn, v); a[0].mx = fmax(a[0].mx, v); a[0].cnt++;
-            if (y >= 1) { a[1].mn = fmin(a[1].mn, v); a[1].mx = fmax(a[1].mx, v); a[1].cnt++; }
+            if (any_masked ? y != 1 : y >= 1) { a[1].mn = fmin(a[1].mn, v); a[1].mx = fmax(a[1].mx, v); a[1].cnt++; }
             if (y >= 2) { a[2].mn = fmin(a[2].mn, v); a[2].mx = fmax(a[2].mx, v); a[2].cnt++; }
         }
         if (dil > 0 && any_masked) {
@@ -180,10 +183,9 @@ quantise_kernel(const double *__restrict__ img, const uint8_t *__restrict__ mask
         const bool any_clear = stats[11] > 0.0;                       // buffered mask contains a 0
         const bool any_masked = stats[2] < (double)m * (double)n;     // ... contains a 1
         if (dil > 0) {
-            const int rows = (any_clear ? 1 : 0) + (any_masked ? 1 : 0);
-            set = rows;  // rows masked from the top: 0, 1 or 2 (row 1 alone only if nothing is clear)
+            // rows masked: row 0, row 1 or both; set 1 is the rows left by either single one
+            set = (any_clear ? 1 : 0) + (any_masked ? 1 : 0);
             if ((y == 0 && any_clear) || (y == 1 && any_masked)) msk = true;
-            if (!any_clear && any_masked) { set = 2; if (y == 0) msk = true; }
         }
     } else if (valid) {
         valid[i] = msk ? 0 : 1;
@@ -317,11 +319,13 @@ constexpr int BOX_R = 64;  // rows in flight per warp: 64 rows * 32 columns * 8 
 
 __device__ __forceinline__ void cp_async8(void *smem_dst, const void *gmem_src) {
     const unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(s), "l"(gmem_src));
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(s), "l"(gmem_src) : "memory");
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+// the ring is read with plain shared loads right after the wait: the "memory" clobbers keep the
+// compiler from moving those loads above it (or the refill's copies above the reads)
 template <int N> __device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
+    asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
 }
 
 // grid = (ceil(w/32), 3): one warp per (32 columns, covariance plane), so the three running

@@ -145,6 +145,8 @@ front_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ F
     const bool opening = p.opening != 0;
     const bool any_masked = p.stats0[2] < (double)m * (double)n;
     const bool buffer = p.dil > 0 && any_masked;
+    // set 1 leaves out row 0, or row 1 when anything is masked (masked_minmax_kernel of lk_dense.cu)
+    const int set1_out = any_masked ? 1 : 0;
     const int dil_lo = -(p.dil / 2), dil_hi = p.dil - 1 - p.dil / 2;
     MM acc[4];
     if (PASS == 1) {
@@ -154,7 +156,7 @@ front_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ F
     Scale sc_track, sc_det;
     double fill = 0.0;
     bool any_clear = false;
-    int det_set = 0;
+    int det_set = 0, det_row0 = -1, det_row1 = -1;   // rows the detector masks: 0 and / or 1, or none
     if (PASS == 2) {
         const double *st = p.stats;
         fill = st[0];
@@ -162,7 +164,8 @@ front_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ F
         // feature/shitomasi.py:131-151 (see quantise_kernel of lk_dense.cu, mode 1)
         if (p.dil > 0) {
             det_set = (any_clear ? 1 : 0) + (any_masked ? 1 : 0);
-            if (!any_clear && any_masked) det_set = 2;
+            det_row0 = any_clear ? 0 : -1;
+            det_row1 = any_masked ? 1 : -1;
         }
         sc_track.init(st, 0);
         sc_det.init(st, det_set);
@@ -241,7 +244,7 @@ front_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ F
             if (PASS == 1) {
                 if (!mk0) {
                     acc[0].mn = fmin(acc[0].mn, v); acc[0].mx = fmax(acc[0].mx, v); acc[0].cnt++;
-                    if (y >= 1) { acc[1].mn = fmin(acc[1].mn, v); acc[1].mx = fmax(acc[1].mx, v); acc[1].cnt++; }
+                    if (y != set1_out) { acc[1].mn = fmin(acc[1].mn, v); acc[1].mx = fmax(acc[1].mx, v); acc[1].cnt++; }
                     if (y >= 2) { acc[2].mn = fmin(acc[2].mn, v); acc[2].mx = fmax(acc[2].mx, v); acc[2].cnt++; }
                 }
                 if (!d) acc[3].cnt++;
@@ -254,10 +257,7 @@ front_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ F
                 if (p.q_det) {
                     if (p.valid) p.valid[i] = d ? 0 : 1;
                     bool mk = mk0;
-                    if (p.dil > 0) {
-                        if ((y == 0 && any_clear) || (y == 1 && any_masked)) mk = true;
-                        if (!any_clear && any_masked && y == 0) mk = true;
-                    }
+                    if (y == det_row0 || y == det_row1) mk = true;
                     const double vd = mk ? fill : v;
                     p.q_det[i] = p.f32 ? cast_u8(qz::scale_f32(vd, sc_det.im_min, sc_det.im_max))
                                        : sc_det(vd);

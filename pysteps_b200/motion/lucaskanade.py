@@ -384,8 +384,10 @@ def dense_lucaskanade(input_images, lk_kwargs=None, fd_method="shitomasi", fd_kw
     # while the side stream prepares the next frame and builds both pyramids.
     main = torch.cuda.current_stream()
     side = _side_stream()
-    # fused, TMA-tiled front end whenever the copy engine can address the frame (16-byte rows)
-    fused = n % 2 == 0 and 0 <= buffer_mask <= 5
+    # fused, TMA-tiled front end whenever the copy engine can address the frame: 16-byte rows and a
+    # 16-byte aligned first frame (then every frame is, m * n * 8 being a multiple of 16).  A view into
+    # a larger tensor can start 8 bytes off; it takes the stage kernels.
+    fused = n % 2 == 0 and 0 <= buffer_mask <= 5 and frames_d.data_ptr() % 16 == 0
     frames = [_Frame(frames_d[t], None if user_mask_d is None else user_mask_d[t], m, n, size_opening, f32,
                      fused, t < nr_fields - 1)
               for t in range(nr_fields)]
