@@ -315,7 +315,11 @@ int b200_detect_outliers_global(const double *uv, const int *n_dev, int n_cap, d
 int b200_compact_rows(const double *xy, const double *uv, const uint8_t *drop, const int *n_dev,
                       int n_cap, double *out_xy, double *out_uv, int *out_count, void *stream);
 /* pysteps/utils/cleansing.py:21-121 decluster(xy, uv, scale, min_samples): per-cell medians,
- * cells in np.unique(axis=0) order. */
+ * cells in np.unique(axis=0) order.  n_cap <= 16384.  As in the reference, a row with a NaN
+ * coordinate belongs to no cell and +-inf coordinates form their own cells (first / last).  Cells
+ * floor(xy / scale) outside [1 - 2^24, 2^24 - 2], and NaN coordinates with min_samples < 1 (the
+ * reference appends a NaN median for each), are refused on the device: *out_count = -1 and nothing
+ * else is written. */
 int b200_decluster(const double *xy, const double *uv, const int *n_dev, int n_cap, double scale,
                    int min_samples, double *out_xy, double *out_uv, int *out_count, void *stream);
 

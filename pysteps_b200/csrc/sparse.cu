@@ -47,6 +47,23 @@ compact_rows_kernel(const double *__restrict__ xy, const double *__restrict__ uv
 
 // ---- decluster ---------------------------------------------------------------------------
 constexpr int DC_MAX = 16384;  // vectors (12 B of shared memory each)
+// key = cell_x code (25 bits) | cell_y code (25 bits) | index (14 bits: DC_MAX - 1 fits).  A finite
+// cell c in [1 - DC_BIAS, DC_BIAS - 2] has code c + DC_BIAS; -inf is code 0 and +inf the largest
+// code, so infinite cells sort where np.unique puts them.
+constexpr int DC_IBITS = 14, DC_CBITS = 25;
+constexpr long long DC_BIAS = 1ll << (DC_CBITS - 1);
+constexpr unsigned long long DC_IMASK = (1ull << DC_IBITS) - 1;
+
+// floor(c / scale) as a key code: -1 for NaN (the row matches no cell), -2 for a finite cell the
+// key cannot hold
+__device__ __forceinline__ long long cell_code(double c, double scale) {
+    const double f = floor(__ddiv_rn(c, scale));
+    if (isnan(f)) return -1;
+    if (f == -CUDART_INF) return 0;
+    if (f == CUDART_INF) return 2 * DC_BIAS - 1;
+    if (f < (double)(1 - DC_BIAS) || f > (double)(DC_BIAS - 2)) return -2;
+    return (long long)f + DC_BIAS;
+}
 
 __device__ __forceinline__ double median_of(const double *__restrict__ a, int stride,
                                             const unsigned long long *__restrict__ keys, int s) {
@@ -54,10 +71,10 @@ __device__ __forceinline__ double median_of(const double *__restrict__ a, int st
     double lo = 0.0, hi = 0.0;
     const int rlo = (s - 1) / 2, rhi = s / 2;
     for (int p = 0; p < s; p++) {
-        const double v = a[(size_t)(keys[p] & 0x3fffff) * stride];
+        const double v = a[(size_t)(keys[p] & DC_IMASK) * stride];
         int rank = 0;
         for (int q = 0; q < s; q++) {
-            const double u = a[(size_t)(keys[q] & 0x3fffff) * stride];
+            const double u = a[(size_t)(keys[q] & DC_IMASK) * stride];
             rank += (u < v) || (u == v && q < p);
         }
         if (rank == rlo) lo = v;
@@ -72,25 +89,38 @@ decluster_kernel(const double *__restrict__ xy, const double *__restrict__ uv, c
                  double *__restrict__ ouv, int *__restrict__ out_count) {
     extern __shared__ __align__(16) unsigned char dc_smem[];
     __shared__ int s_nseg;
-    const int n = n_dev ? min(*n_dev, n_cap) : n_cap;
+    const int ncap = n_dev ? min(*n_dev, n_cap) : n_cap;
     const int tid = threadIdx.x;
     int npad = 1;
-    while (npad < n) npad <<= 1;
+    while (npad < ncap) npad <<= 1;
     if (npad < 2) npad = 2;
     unsigned long long *key = reinterpret_cast<unsigned long long *>(dc_smem);  // cap_pad entries
     int *seg_start = reinterpret_cast<int *>(key + cap_pad);                    // cap_pad + 1
-    // key = (cell_x, cell_y, index): np.unique(axis=0) orders cells lexicographically by x then y
+    // key = (cell_x, cell_y, index): np.unique(axis=0) orders cells lexicographically by x then y.
+    // A row with a NaN cell matches no cell of the reference (coord_ == ucoord_ is false): it sorts
+    // last, past the n rows that count.
+    __shared__ int s_nan;
+    if (tid == 0) s_nan = 0;
+    __syncthreads();
+    int refuse = 0;
     for (int i = tid; i < npad; i += blockDim.x) {
         unsigned long long kv = ~0ull;
-        if (i < n) {
-            const long long cx = (long long)floor(__ddiv_rn(xy[2 * i], scale)) + (1 << 20);
-            const long long cy = (long long)floor(__ddiv_rn(xy[2 * i + 1], scale)) + (1 << 20);
-            kv = ((unsigned long long)(cx & 0x1fffff) << 43) | ((unsigned long long)(cy & 0x1fffff) << 22) |
-                 (unsigned long long)i;
+        if (i < ncap) {
+            const long long cx = cell_code(xy[2 * i], scale), cy = cell_code(xy[2 * i + 1], scale);
+            if (cx == -2 || cy == -2) refuse = 1;
+            else if (cx == -1 || cy == -1) atomicAdd(&s_nan, 1);
+            else kv = ((unsigned long long)cx << (DC_CBITS + DC_IBITS)) | ((unsigned long long)cy << DC_IBITS) |
+                      (unsigned long long)i;
         }
         key[i] = kv;
     }
-    __syncthreads();
+    // a cell beyond the key, or NaN rows where the reference appends a NaN median for each of them
+    // (min_samples < 1): refused with *out_count = -1, nothing else written
+    if (__syncthreads_or(refuse) || (s_nan > 0 && min_samples < 1)) {
+        if (tid == 0) *out_count = -1;
+        return;
+    }
+    const int n = ncap - s_nan;
     for (int k = 2; k <= npad; k <<= 1)
         for (int j = k >> 1; j > 0; j >>= 1) {
             for (int t = tid; t < npad / 2; t += blockDim.x) {
@@ -109,7 +139,7 @@ decluster_kernel(const double *__restrict__ xy, const double *__restrict__ uv, c
         int local = 0;
         for (int q = 0; q < per; q++) {
             const int i = i0 + q;
-            if (i < n && (i == 0 || (key[i] >> 22) != (key[i - 1] >> 22))) local++;
+            if (i < n && (i == 0 || (key[i] >> DC_IBITS) != (key[i - 1] >> DC_IBITS))) local++;
         }
         int incl = local;
         const int lane = tid & 31, wid = tid >> 5;
@@ -125,7 +155,7 @@ decluster_kernel(const double *__restrict__ xy, const double *__restrict__ uv, c
         int pos = base + incl - local;  // number of heads before this thread's elements
         for (int q = 0; q < per; q++) {
             const int i = i0 + q;
-            if (i < n && (i == 0 || (key[i] >> 22) != (key[i - 1] >> 22))) seg_start[pos++] = i;
+            if (i < n && (i == 0 || (key[i] >> DC_IBITS) != (key[i - 1] >> DC_IBITS))) seg_start[pos++] = i;
         }
         if (tid == (int)blockDim.x - 1) {
             s_nseg = base + incl;

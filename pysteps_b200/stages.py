@@ -201,6 +201,9 @@ def decluster(coord, input_array, scale, min_samples=1, verbose=False):
     _lib.call("b200_decluster", dxy.data_ptr(), duv.data_ptr(), None, n, float(scale), int(min_samples),
               oxy.data_ptr(), ouv.data_ptr(), cnt.data_ptr(), _s())
     c = int(cnt.item())
+    if c < 0:
+        raise ValueError("pysteps_b200 decluster: a cell floor(coord / scale) lies outside [1 - 2**24, 2**24 - 2], "
+                         "or coord has NaN values and min_samples < 1")
     if verbose:
         print("--- %i samples left after declustering ---" % c)
     return oxy[:c].cpu().numpy(), ouv[:c].cpu().numpy()

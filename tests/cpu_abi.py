@@ -410,6 +410,12 @@ def _lk_decluster(xy, uv, n_dev, cap, scale, min_samples, oxy, ouv, ocount, stre
     from oracle import lucaskanade as ora_lk
     cnt = _count(n_dev, cap)
     k = 0
+    with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+        cells = np.floor(_view(xy, (cap, 2))[:cnt] / float(scale))
+    finite = cells[np.isfinite(cells)]
+    if np.any((finite < 1 - 2 ** 24) | (finite > 2 ** 24 - 2)) or (np.isnan(cells).any() and min_samples < 1):
+        _view(ocount, (1,), np.int32)[0] = -1  # refused (csrc/sparse.cu cell_code)
+        return
     if cnt:
         dxy, duv = ora_lk.decluster(_view(xy, (cap, 2))[:cnt].copy(), _view(uv, (cap, 2))[:cnt].copy(), scale,
                                     min_samples)
