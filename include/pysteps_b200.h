@@ -728,6 +728,41 @@ int b200_fss_fractions(const void *X, int dtype, int nf, int m, int n, double th
  * enqueues kernels. */
 int b200_fss_sums(const double *S, int64_t P, int a0, int na, int b0, int nb, double *out, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Probability matching (pysteps/postprocessing/probmatching.py).  Device memory unless stated
+ * otherwise; dtypes B200_F32 / B200_F64; n < 2^31.  Ties are ranked in index order, as
+ * argsort(kind="stable") ranks them.  Only enqueue kernels. */
+
+/* Device scratch of b200_pm_match_stats, b200_pm_match and b200_pm_resample for n values. */
+int b200_pm_scratch_bytes(int64_t n, int64_t *bytes);
+
+/* stats (8 doubles) of nonparam_match_empirical_cdf's initial array x (n_x values, ignore: n_x bytes,
+ * nonzero where ignored, or NULL) and target t (n_t values): [0] np.nanmin(x) (NaN when every x is
+ * NaN), [1] the non-NaN x, [2] the non-finite x outside the mask, [3] the x inside it, [4] the x >
+ * stats[0] outside it, [5] np.nanmin(t), [6] the non-NaN t, [7] the t > stats[5].  A zero minimum is
+ * -0.0 when some minimal value is -0.0. */
+int b200_pm_match_stats(const void *x, int x_dtype, const unsigned char *ignore, int64_t n_x, const void *t,
+                        int t_dtype, int64_t n_t, double *stats, void *scratch, int64_t scratch_bytes, void *stream);
+
+/* out (n float64) = nonparam_match_empirical_cdf(x, t, ignore) from the stats of b200_pm_match_stats
+ * (stats[2] must be 0); n_xwet = stats[4] and n_twet = stats[7] as integers.  clip: the values of t
+ * below p = _lerp(s[i0], s[i1], gamma) of the sorted t (NaN as stats[5]) become stats[5]. */
+int b200_pm_match(const void *x, int x_dtype, const unsigned char *ignore, const void *t, int t_dtype, int64_t n,
+                  const double *stats, int64_t n_xwet, int64_t n_twet, int clip, int64_t i0, int64_t i1,
+                  double gamma, double *out, void *scratch, int64_t scratch_bytes, void *stream);
+
+/* *n_nan (int64) = the indices i < n where a[i] or b[i] is NaN. */
+int b200_pm_resample_nan(const void *a, int a_dtype, const void *b, int b_dtype, int64_t n, int64_t *n_nan,
+                         void *stream);
+
+/* out (n of out_dtype) = resample_distributions(a, b): n_nan (from b200_pm_resample_nan) NaNs, then
+ * the values that are NaN in neither array, sorted in descending order, position n_nan + q taken
+ * from a where draws[n_nan + q] (n bytes, 0 or 1) is nonzero and from b elsewhere, sorted again in
+ * descending order. */
+int b200_pm_resample(const void *a, int a_dtype, const void *b, int b_dtype, int64_t n, int64_t n_nan,
+                     const unsigned char *draws, void *out, int out_dtype, void *scratch, int64_t scratch_bytes,
+                     void *stream);
+
 #ifdef __cplusplus
 }
 #endif

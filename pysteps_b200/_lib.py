@@ -165,6 +165,14 @@ _SIGNATURES = {
     "b200_fss_fractions": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_int, c_void_p,
                                    c_void_p]),
     "b200_fss_sums": (c_int, [c_void_p, c_i64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "b200_pm_scratch_bytes": (c_int, [c_i64, ctypes.POINTER(c_i64)]),
+    "b200_pm_match_stats": (c_int, [c_void_p, c_int, c_void_p, c_i64, c_void_p, c_int, c_i64, c_void_p, c_void_p,
+                                    c_i64, c_void_p]),
+    "b200_pm_match": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_i64, c_void_p, c_i64, c_i64, c_int, c_i64,
+                              c_i64, c_double, c_void_p, c_void_p, c_i64, c_void_p]),
+    "b200_pm_resample_nan": (c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p, c_void_p]),
+    "b200_pm_resample": (c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_i64, c_void_p, c_void_p, c_int, c_void_p,
+                                 c_i64, c_void_p]),
 }
 
 

@@ -10,25 +10,14 @@
 //              through the member maps, the NWP is nan_to_num'd, the nowcast's NaN filled per output
 //              member, and each lead copied or blended in the dtypes the host passes (no FMA).
 //   salient    per lead: maxima of both slabs (integer atomics on order-preserving keys), diff and
-//              its 64-bit keys, an LSD radix sort of (key, index) pairs in 8-bit digits that skips
-//              every digit all keys share, a dense rank from an inclusive scan of key changes
+//              its 64-bit keys, the LSD radix sort of radix_sort.cuh (8-bit digits, every digit all
+//              keys share skipped), a dense rank from an inclusive scan of key changes
 //              scattered back to pixel order, then the salience weight and the blended value.
 // No atomics touch floating-point values and every scan runs in a fixed order, so repeated calls
 // are bit-identical.
-#include <algorithm>
-
-#include "common.cuh"
+#include "radix_sort.cuh"
 
 namespace {
-
-constexpr int THREADS = 256;
-constexpr int SORT_ITEMS = 16;
-constexpr int TILE = THREADS * SORT_ITEMS;  // keys per radix tile and per scan block
-constexpr int RADIX = 256;
-constexpr int PASSES = 8;
-constexpr unsigned FULL = 0xffffffffu;
-
-__device__ __forceinline__ double quiet_nan() { return __longlong_as_double(0x7ff8000000000000ll); }
 
 template <typename T> __device__ __forceinline__ T max_finite();
 template <> __device__ __forceinline__ float max_finite<float>() { return 3.4028234663852886e38f; }
@@ -39,16 +28,6 @@ template <typename T> __device__ __forceinline__ T nan_to_num(T v) {
     if (isnan(v)) return T(0);
     if (isinf(v)) return v > T(0) ? max_finite<T>() : -max_finite<T>();
     return v;
-}
-
-// order-preserving 64-bit image of a double; -0.0 maps to +0.0 (rankdata treats them as equal)
-__device__ __forceinline__ unsigned long long order_key(double d) {
-    unsigned long long u = (unsigned long long)__double_as_longlong(d == 0.0 ? 0.0 : d);
-    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
-}
-__device__ __forceinline__ double key_value(unsigned long long k) {
-    if (k == ~0ull) return quiet_nan();
-    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
 }
 
 // ---------------------------------------------------------------- conversion to rain rate
@@ -167,43 +146,21 @@ __global__ void __launch_bounds__(THREADS)
 
 // ---------------------------------------------------------------- salience: maxima, diff, keys
 struct SortScratch {
-    unsigned long long *key[2];
-    unsigned *idx[2];
-    unsigned *tiles;  // RADIX x n_tiles digit counts, digit-major, then their exclusive scan
-    unsigned *bsum;   // per scan block sums
-    unsigned *rank;   // dense rank of every pixel
-    unsigned *ghist;  // PASSES x RADIX global digit counts
-    int *src;         // PASSES + 1: buffer each pass reads (-1: pass skipped); [PASSES]: the final buffer
+    SortBuffers sort;
+    unsigned *rank;              // dense rank of every pixel
     unsigned long long *maxkey;  // 2: maxima of the two slabs
     int *nan_flag;
     unsigned *max_rank;
 };
 
-static int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
-
 static int64_t carve(SortScratch *s, char *base, int64_t n) {
-    const int64_t n_tiles = b200::ceil_div64(std::max<int64_t>(n, 1), TILE);
-    const int64_t n_scan = std::max<int64_t>(RADIX * n_tiles, n);
-    const int64_t n_bsum = b200::ceil_div64(n_scan, TILE);
-    int64_t off = 0;
-    auto take = [&](int64_t bytes) {
-        char *p = base ? base + off : nullptr;
-        off += align256(bytes);
-        return p;
-    };
-    s->key[0] = (unsigned long long *)take(8 * n);
-    s->key[1] = (unsigned long long *)take(8 * n);
-    s->idx[0] = (unsigned *)take(4 * n);
-    s->idx[1] = (unsigned *)take(4 * n);
-    s->tiles = (unsigned *)take(4 * RADIX * n_tiles);
-    s->bsum = (unsigned *)take(4 * n_bsum);
-    s->rank = (unsigned *)take(4 * n);
-    s->ghist = (unsigned *)take(4 * PASSES * RADIX);
-    s->src = (int *)take(4 * (PASSES + 1));
-    s->maxkey = (unsigned long long *)take(16);
-    s->nan_flag = (int *)take(4);
-    s->max_rank = (unsigned *)take(4);
-    return off;
+    Carver c{base};
+    carve_sort(&s->sort, c, n);
+    s->rank = (unsigned *)c.take(4 * n);
+    s->maxkey = (unsigned long long *)c.take(16);
+    s->nan_flag = (int *)c.take(4);
+    s->max_rank = (unsigned *)c.take(4);
+    return c.off;
 }
 
 // warp max of 64-bit values (no 64-bit redux instruction)
@@ -268,224 +225,27 @@ __global__ void __launch_bounds__(THREADS)
     if (__any_sync(FULL, nan_seen) && (threadIdx.x & 31) == 0) atomicOr(nan_flag, 1);
 }
 
-// ---------------------------------------------------------------- radix sort
-__global__ void __launch_bounds__(THREADS)
-    global_hist(const unsigned long long *__restrict__ key, int64_t n, unsigned *__restrict__ ghist) {
-    __shared__ unsigned h[PASSES][RADIX];
-    for (int t = threadIdx.x; t < PASSES * RADIX; t += THREADS) (&h[0][0])[t] = 0;
-    __syncthreads();
-    for (int64_t j = (int64_t)blockIdx.x * THREADS + threadIdx.x; j < n; j += (int64_t)gridDim.x * THREADS) {
-        const unsigned long long k = key[j];
-#pragma unroll
-        for (int d = 0; d < PASSES; d++) atomicAdd(&h[d][(k >> (8 * d)) & 255], 1u);
-    }
-    __syncthreads();
-    for (int t = threadIdx.x; t < PASSES * RADIX; t += THREADS)
-        if ((&h[0][0])[t]) atomicAdd(ghist + t, (&h[0][0])[t]);
-}
-
-// src[d]: the buffer pass d reads, or -1 when every key has the same digit d (the pass is skipped)
-__global__ void plan_passes(const unsigned *__restrict__ ghist, int64_t n, int *__restrict__ src) {
-    if (threadIdx.x != 0) return;
-    int cur = 0;
-    for (int d = 0; d < PASSES; d++) {
-        bool trivial = false;
-        for (int b = 0; b < RADIX; b++) trivial |= (int64_t)ghist[d * RADIX + b] == n;
-        src[d] = trivial ? -1 : cur;
-        if (!trivial) cur ^= 1;
-    }
-    src[PASSES] = cur;
-}
-
-__global__ void __launch_bounds__(THREADS)
-    tile_hist(SortScratch s, int64_t n, int64_t n_tiles, int pass) {
-    const int b = s.src[pass];
-    if (b < 0) return;
-    __shared__ unsigned h[RADIX];
-    h[threadIdx.x] = 0;
-    __syncthreads();
-    const unsigned long long *key = s.key[b];
-    const int64_t t0 = (int64_t)blockIdx.x * TILE;
-    for (int r = 0; r < SORT_ITEMS; r++) {
-        const int64_t j = t0 + r * THREADS + threadIdx.x;
-        if (j < n) atomicAdd(&h[(key[j] >> (8 * pass)) & 255], 1u);
-    }
-    __syncthreads();
-    s.tiles[(int64_t)threadIdx.x * n_tiles + blockIdx.x] = h[threadIdx.x];
-}
-
-// block-wide exclusive scan of one value per thread; returns the total in *total
-__device__ __forceinline__ unsigned block_exclusive(unsigned v, unsigned *total) {
-    __shared__ unsigned warp_sum[THREADS / 32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned y = __shfl_up_sync(FULL, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) warp_sum[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        unsigned s = lane < THREADS / 32 ? warp_sum[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned y = __shfl_up_sync(FULL, s, o);
-            if (lane >= o) s += y;
-        }
-        if (lane < THREADS / 32) warp_sum[lane] = s;
-    }
-    __syncthreads();
-    const unsigned before = (w ? warp_sum[w - 1] : 0) + x - v;
-    *total = warp_sum[THREADS / 32 - 1];
-    __syncthreads();
-    return before;
-}
-
-// the scans: over the tile counts of a pass (exclusive, in place), or over the key changes of the
-// sorted keys (inclusive: the dense rank, scattered to pixel order)
-struct CountScan {
-    SortScratch s;
-    int pass;
-    __device__ bool skip() const { return s.src[pass] < 0; }
-    __device__ unsigned load(int64_t i) const { return s.tiles[i]; }
-    __device__ void store(int64_t i, unsigned excl, unsigned) const { s.tiles[i] = excl; }
-};
+// ---------------------------------------------------------------- dense rank
+// the inclusive scan of the key changes of the sorted keys: the dense rank, scattered to pixel order
 struct RankScan {
     SortScratch s;
     int64_t n;
     __device__ bool skip() const { return false; }
     __device__ unsigned load(int64_t i) const {
-        const unsigned long long *k = s.key[s.src[PASSES]];
+        const unsigned long long *k = s.sort.key[s.sort.src[PASSES]];
         return i == 0 || k[i] != k[i - 1];
     }
     __device__ void store(int64_t i, unsigned excl, unsigned v) const {
         const unsigned incl = excl + v;
-        s.rank[s.idx[s.src[PASSES]][i]] = incl;
+        s.rank[s.sort.idx[s.sort.src[PASSES]][i]] = incl;
         if (i == n - 1) *s.max_rank = incl;
     }
 };
 
-template <typename Op>
-__global__ void __launch_bounds__(THREADS) scan_reduce(Op op, int64_t n, unsigned *__restrict__ bsum) {
-    if (op.skip()) return;
-    const int64_t i0 = (int64_t)blockIdx.x * TILE + (int64_t)threadIdx.x * SORT_ITEMS;
-    unsigned v = 0;
-    for (int r = 0; r < SORT_ITEMS; r++)
-        if (i0 + r < n) v += op.load(i0 + r);
-    unsigned total;
-    block_exclusive(v, &total);
-    if (threadIdx.x == 0) bsum[blockIdx.x] = total;
-}
-
-template <typename Op>
-__global__ void __launch_bounds__(THREADS) scan_blocks(Op op, int64_t nb, unsigned *__restrict__ bsum) {
-    if (op.skip()) return;
-    unsigned carry = 0;
-    for (int64_t b0 = 0; b0 < nb; b0 += THREADS) {
-        const int64_t b = b0 + threadIdx.x;
-        const unsigned v = b < nb ? bsum[b] : 0;
-        unsigned total;
-        const unsigned e = block_exclusive(v, &total);
-        if (b < nb) bsum[b] = carry + e;
-        carry += total;
-    }
-}
-
-template <typename Op>
-__global__ void __launch_bounds__(THREADS) scan_apply(Op op, int64_t n, const unsigned *__restrict__ bsum) {
-    if (op.skip()) return;
-    const int64_t i0 = (int64_t)blockIdx.x * TILE + (int64_t)threadIdx.x * SORT_ITEMS;
-    unsigned v[SORT_ITEMS];
-    unsigned sum = 0;
-#pragma unroll
-    for (int r = 0; r < SORT_ITEMS; r++) {
-        v[r] = i0 + r < n ? op.load(i0 + r) : 0;
-        sum += v[r];
-    }
-    unsigned total;
-    unsigned run = bsum[blockIdx.x] + block_exclusive(sum, &total);
-#pragma unroll
-    for (int r = 0; r < SORT_ITEMS; r++) {
-        if (i0 + r < n) op.store(i0 + r, run, v[r]);
-        run += v[r];
-    }
-}
-
-// stable scatter of one tile: keys are taken in index order, ranked within their warp by
-// __match_any_sync and across the warps of a round by a per-digit scan in shared memory
-__global__ void __launch_bounds__(THREADS) scatter_pass(SortScratch s, int64_t n, int64_t n_tiles, int pass) {
-    const int b = s.src[pass];
-    if (b < 0) return;
-    __shared__ unsigned base[RADIX];
-    __shared__ unsigned wcnt[THREADS / 32][RADIX];
-    __shared__ unsigned round_total[RADIX];
-    const unsigned long long *ksrc = s.key[b];
-    const unsigned *isrc = s.idx[b];
-    unsigned long long *kdst = s.key[b ^ 1];
-    unsigned *idst = s.idx[b ^ 1];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    base[threadIdx.x] = s.tiles[(int64_t)threadIdx.x * n_tiles + blockIdx.x];
-    const int64_t t0 = (int64_t)blockIdx.x * TILE;
-    for (int r = 0; r < SORT_ITEMS; r++) {
-        for (int q = 0; q < THREADS / 32; q++) wcnt[q][threadIdx.x] = 0;
-        __syncthreads();
-        const int64_t j = t0 + (int64_t)r * THREADS + threadIdx.x;
-        const bool valid = j < n;
-        const unsigned long long k = valid ? ksrc[j] : 0ull;
-        const unsigned digit = valid ? (unsigned)((k >> (8 * pass)) & 255) : RADIX + lane;
-        const unsigned peers = __match_any_sync(FULL, digit);
-        const unsigned below = __popc(peers & ((1u << lane) - 1u));
-        if (valid && below == 0) wcnt[w][digit] = __popc(peers);
-        __syncthreads();
-        unsigned acc = 0;
-        for (int q = 0; q < THREADS / 32; q++) {
-            const unsigned c = wcnt[q][threadIdx.x];
-            wcnt[q][threadIdx.x] = acc;
-            acc += c;
-        }
-        round_total[threadIdx.x] = acc;
-        __syncthreads();
-        if (valid) {
-            const unsigned pos = base[digit] + wcnt[w][digit] + below;
-            kdst[pos] = k;
-            idst[pos] = isrc[j];
-        }
-        __syncthreads();
-        base[threadIdx.x] += round_total[threadIdx.x];
-    }
-}
-
-int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(b200::ceil_div64(n, THREADS), 132 * 16)); }
-
-// sort the n keys in s.key[0] / s.idx[0] and rank them densely into s.rank, s.max_rank
+// sort the n keys in s.sort.key[0] / s.sort.idx[0] and rank them densely into s.rank, s.max_rank
 int dense_rank(SortScratch &s, int64_t n, cudaStream_t st) {
-    const int64_t n_tiles = b200::ceil_div64(n, TILE);
-    B200_CUDA(cudaMemsetAsync(s.ghist, 0, 4 * PASSES * RADIX, st));
-    global_hist<<<grid_for(n), THREADS, 0, st>>>(s.key[0], n, s.ghist);
-    B200_LAUNCH_CHECK();
-    plan_passes<<<1, 32, 0, st>>>(s.ghist, n, s.src);
-    B200_LAUNCH_CHECK();
-    const int64_t n_counts = RADIX * n_tiles;
-    const int64_t nb = b200::ceil_div64(n_counts, TILE);
-    for (int d = 0; d < PASSES; d++) {
-        tile_hist<<<(unsigned)n_tiles, THREADS, 0, st>>>(s, n, n_tiles, d);
-        B200_LAUNCH_CHECK();
-        scan_reduce<<<(unsigned)nb, THREADS, 0, st>>>(CountScan{s, d}, n_counts, s.bsum);
-        B200_LAUNCH_CHECK();
-        scan_blocks<<<1, THREADS, 0, st>>>(CountScan{s, d}, nb, s.bsum);
-        B200_LAUNCH_CHECK();
-        scan_apply<<<(unsigned)nb, THREADS, 0, st>>>(CountScan{s, d}, n_counts, s.bsum);
-        B200_LAUNCH_CHECK();
-        scatter_pass<<<(unsigned)n_tiles, THREADS, 0, st>>>(s, n, n_tiles, d);
-        B200_LAUNCH_CHECK();
-    }
-    const int64_t rb = b200::ceil_div64(n, TILE);
-    scan_reduce<<<(unsigned)rb, THREADS, 0, st>>>(RankScan{s, n}, n, s.bsum);
-    B200_LAUNCH_CHECK();
-    scan_blocks<<<1, THREADS, 0, st>>>(RankScan{s, n}, rb, s.bsum);
-    B200_LAUNCH_CHECK();
-    scan_apply<<<(unsigned)rb, THREADS, 0, st>>>(RankScan{s, n}, n, s.bsum);
-    B200_LAUNCH_CHECK();
-    return 0;
+    if (int rc = radix_sort(s.sort, n, st)) return rc;
+    return scan(RankScan{s, n}, n, s.sort.bsum, st);
 }
 
 // linear_blending.py:_get_ws on the dense rank, then ws * nowcast + (1 - ws) * nwp in float64;
@@ -544,7 +304,7 @@ int salient_run(const Fields &f, void *out, int n_out, int T, int lead, double w
     B200_CUDA(cudaMemsetAsync(s.nan_flag, 0, 4, st));
     slab_max<Tc, Tn><<<grid_for(n), THREADS, 0, st>>>(f, n_out, lead, s.maxkey);
     B200_LAUNCH_CHECK();
-    diff_keys<Tc, Tn, Td><<<grid_for(n), THREADS, 0, st>>>(f, n_out, lead, s.maxkey, s.key[0], s.idx[0], s.nan_flag);
+    diff_keys<Tc, Tn, Td><<<grid_for(n), THREADS, 0, st>>>(f, n_out, lead, s.maxkey, s.sort.key[0], s.sort.idx[0], s.nan_flag);
     B200_LAUNCH_CHECK();
     if (int rc = dense_rank(s, n, st)) return rc;
     salient_kernel<Tc, Tn><<<grid_for(n), THREADS, 0, st>>>(f, (Tn *)out, n_out, T, lead, s, w, w1, w2, w12);
@@ -667,8 +427,8 @@ extern "C" int b200_dense_rank(const void *x, int dtype, int64_t n, unsigned *ra
     carve(&s, (char *)scratch, n);
     cudaStream_t st = (cudaStream_t)stream;
     B200_CUDA(cudaMemsetAsync(s.nan_flag, 0, 4, st));
-    if (dtype == B200_F32) array_keys<float><<<grid_for(n), THREADS, 0, st>>>((const float *)x, n, s.key[0], s.idx[0], s.nan_flag);
-    else if (dtype == B200_F64) array_keys<double><<<grid_for(n), THREADS, 0, st>>>((const double *)x, n, s.key[0], s.idx[0], s.nan_flag);
+    if (dtype == B200_F32) array_keys<float><<<grid_for(n), THREADS, 0, st>>>((const float *)x, n, s.sort.key[0], s.sort.idx[0], s.nan_flag);
+    else if (dtype == B200_F64) array_keys<double><<<grid_for(n), THREADS, 0, st>>>((const double *)x, n, s.sort.key[0], s.sort.idx[0], s.nan_flag);
     else {
         b200::set_error("dense_rank: dtype must be B200_F32 or B200_F64");
         return B200_EINVAL;
