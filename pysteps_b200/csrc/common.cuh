@@ -1,4 +1,5 @@
-// common.cuh -- shared helpers for libpysteps_b200.so (sm_90a only).
+// common.cuh -- shared helpers for libpysteps_b200.so (sm_90a only): error reporting, scratch
+// allocation and carving, and small device helpers that restate NumPy and OpenCV conventions.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -52,5 +53,33 @@ struct Scratch {
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
+static inline int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
+
+// consecutive 256-byte aligned pieces of one scratch allocation; base == nullptr only sizes them
+struct Carver {
+    char *base;
+    int64_t off = 0;
+    void *take(int64_t bytes) {
+        char *p = base ? base + off : nullptr;
+        off += align256(bytes);
+        return p;
+    }
+};
+
+__device__ __forceinline__ double quiet_nan() { return __longlong_as_double(0x7ff8000000000000ll); }
+
+// the dtype NumPy computes a difference of an F and an O in
+template <typename F, typename O> struct Promote { using T = double; };
+template <> struct Promote<float, float> { using T = float; };
+
+// OpenCV's BORDER_REFLECT_101: the index of i reflected into [0, L) without repeating the edge
+__device__ __forceinline__ int reflect101(int i, int L) {
+    if (L == 1) return 0;
+    while (i < 0 || i >= L) {
+        if (i < 0) i = -i;
+        if (i >= L) i = 2 * L - 2 - i;
+    }
+    return i;
+}
 
 }  // namespace b200

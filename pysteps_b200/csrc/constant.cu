@@ -13,6 +13,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "scan.cuh"
 #include "spline_body.cuh"
 
 namespace {
@@ -29,31 +30,32 @@ constexpr int CHUNK = 64;  // below the root every leaf holds >= 64 values: one 
 constexpr int SUM_THREADS = 256, SUM_LANES = B200_CONST_SUM_BLOCKS * SUM_THREADS;
 constexpr int MAX_DEPTH = 40;
 
+// the pieces of one evaluation's scratch, carved from scratch (nullptr: only their size in bytes)
 struct Layout {
-    int64_t P, tiles, chunks;
-    size_t tile_count, tile_off, count, means, part, a, b, leafval, nodeval, arrive, bytes;
+    int64_t P, tiles, chunks, bytes;
+    int *tile_count, *tile_off;
+    long long *count;
+    double *means, *part, *a, *b, *leafval, *nodeval;
+    unsigned *arrive;
 };
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-Layout layout(int m, int n) {
+Layout layout(int m, int n, char *scratch) {
     Layout L;
     L.P = (int64_t)m * n;
     L.tiles = b200::ceil_div64(L.P, TILE);
     L.chunks = std::max<int64_t>(1, b200::ceil_div64(L.P, CHUNK));
-    size_t at = 0;
-    auto take = [&at](size_t bytes) { const size_t here = at; at = align256(at + bytes); return here; };
-    L.tile_count = take(sizeof(int) * L.tiles);
-    L.tile_off = take(sizeof(int) * L.tiles);
-    L.count = take(sizeof(long long));
-    L.means = take(2 * sizeof(double));
-    L.part = take(3 * sizeof(double) * B200_CONST_SUM_BLOCKS);
-    L.a = take(sizeof(double) * L.P);
-    L.b = take(sizeof(double) * L.P);
-    L.leafval = take(2 * sizeof(double) * L.chunks);
-    L.nodeval = take(2 * sizeof(double) * L.chunks);
-    L.arrive = take(sizeof(unsigned) * L.chunks);
-    L.bytes = at;
+    b200::Carver c{scratch};
+    L.tile_count = (int *)c.take(sizeof(int) * L.tiles);
+    L.tile_off = (int *)c.take(sizeof(int) * L.tiles);
+    L.count = (long long *)c.take(sizeof(long long));
+    L.means = (double *)c.take(2 * sizeof(double));
+    L.part = (double *)c.take(3 * sizeof(double) * B200_CONST_SUM_BLOCKS);
+    L.a = (double *)c.take(sizeof(double) * L.P);
+    L.b = (double *)c.take(sizeof(double) * L.P);
+    L.leafval = (double *)c.take(2 * sizeof(double) * L.chunks);
+    L.nodeval = (double *)c.take(2 * sizeof(double) * L.chunks);
+    L.arrive = (unsigned *)c.take(sizeof(unsigned) * L.chunks);
+    L.bytes = c.off;
     return L;
 }
 
@@ -79,32 +81,6 @@ __device__ __forceinline__ bool counted(const Eval &e, int64_t p, double &va, do
     return true;
 }
 
-// exclusive prefix of v over the CTA; *total = the CTA's sum.  sh: THREADS / 32 ints of shared memory
-template <int THREADS>
-__device__ __forceinline__ int block_exclusive_scan(int v, int *sh, int *total) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    int x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) sh[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        int s = lane < THREADS / 32 ? sh[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, s, o);
-            if (lane >= o) s += y;
-        }
-        if (lane < THREADS / 32) sh[lane] = s;
-    }
-    __syncthreads();
-    const int before = w ? sh[w - 1] : 0;
-    *total = sh[THREADS / 32 - 1];
-    __syncthreads();  // sh may be reused by the caller
-    return before + x - v;
-}
-
 template <typename F>
 __global__ void __launch_bounds__(TILE_THREADS) count_kernel(const Eval e, int64_t P, int *__restrict__ tile_count) {
     __shared__ int sh[TILE_THREADS / 32];
@@ -115,7 +91,7 @@ __global__ void __launch_bounds__(TILE_THREADS) count_kernel(const Eval e, int64
         if (base + k < P && counted<F>(e, base + k, a, b)) c++;
     }
     int total;
-    block_exclusive_scan<TILE_THREADS>(c, sh, &total);
+    b200::block_exclusive_scan<TILE_THREADS>(c, sh, &total);
     if (threadIdx.x == 0) tile_count[blockIdx.x] = total;
 }
 
@@ -128,7 +104,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(const int *__restric
     int s = 0;
     for (int64_t t = lo; t < hi; t++) s += tile_count[t];
     int total;
-    int run = block_exclusive_scan<SCAN_THREADS>(s, sh, &total);
+    int run = b200::block_exclusive_scan<SCAN_THREADS>(s, sh, &total);
     for (int64_t t = lo; t < hi; t++) {
         tile_off[t] = run;
         run += tile_count[t];
@@ -149,7 +125,7 @@ __global__ void __launch_bounds__(TILE_THREADS) compact_kernel(const Eval e, int
         c += ok[k];
     }
     int total;
-    int64_t rank = (int64_t)tile_off[blockIdx.x] + block_exclusive_scan<TILE_THREADS>(c, sh, &total);
+    int64_t rank = (int64_t)tile_off[blockIdx.x] + b200::block_exclusive_scan<TILE_THREADS>(c, sh, &total);
     for (int k = 0; k < PER_THREAD; k++)
         if (ok[k]) {
             ra[rank] = va[k];
@@ -335,29 +311,23 @@ __global__ void tail_kernel(const long long *__restrict__ count, const double *_
 }
 
 template <typename F>
-int eval(const Eval &e, const Layout &L, char *scratch, double *record, cudaStream_t s) {
-    int *tile_count = (int *)(scratch + L.tile_count), *tile_off = (int *)(scratch + L.tile_off);
-    long long *count = (long long *)(scratch + L.count);
-    double *means = (double *)(scratch + L.means), *part = (double *)(scratch + L.part);
-    double *ra = (double *)(scratch + L.a), *rb = (double *)(scratch + L.b);
-    double *leafval = (double *)(scratch + L.leafval), *nodeval = (double *)(scratch + L.nodeval);
-    unsigned *arrive = (unsigned *)(scratch + L.arrive);
+int eval(const Eval &e, const Layout &L, double *record, cudaStream_t s) {
     if (L.tiles > 0) {
-        count_kernel<F><<<(unsigned)L.tiles, TILE_THREADS, 0, s>>>(e, L.P, tile_count);
+        count_kernel<F><<<(unsigned)L.tiles, TILE_THREADS, 0, s>>>(e, L.P, L.tile_count);
         B200_LAUNCH_CHECK();
     }
-    scan_kernel<<<1, SCAN_THREADS, 0, s>>>(tile_count, L.tiles, tile_off, count);
+    scan_kernel<<<1, SCAN_THREADS, 0, s>>>(L.tile_count, L.tiles, L.tile_off, L.count);
     B200_LAUNCH_CHECK();
     if (L.tiles > 0) {
-        compact_kernel<F><<<(unsigned)L.tiles, TILE_THREADS, 0, s>>>(e, L.P, tile_off, ra, rb);
+        compact_kernel<F><<<(unsigned)L.tiles, TILE_THREADS, 0, s>>>(e, L.P, L.tile_off, L.a, L.b);
         B200_LAUNCH_CHECK();
     }
-    mean_kernel<<<(unsigned)b200::ceil_div64(L.chunks, 256), 256, 0, s>>>(ra, rb, count, L.chunks, leafval, nodeval,
-                                                                           arrive, means);
+    mean_kernel<<<(unsigned)b200::ceil_div64(L.chunks, 256), 256, 0, s>>>(L.a, L.b, L.count, L.chunks, L.leafval,
+                                                                           L.nodeval, L.arrive, L.means);
     B200_LAUNCH_CHECK();
-    centred_kernel<<<B200_CONST_SUM_BLOCKS, SUM_THREADS, 0, s>>>(ra, rb, count, means, part);
+    centred_kernel<<<B200_CONST_SUM_BLOCKS, SUM_THREADS, 0, s>>>(L.a, L.b, L.count, L.means, L.part);
     B200_LAUNCH_CHECK();
-    tail_kernel<<<1, 1, 0, s>>>(count, part, record);
+    tail_kernel<<<1, 1, 0, s>>>(L.count, L.part, record);
     B200_LAUNCH_CHECK();
     return 0;
 }
@@ -367,7 +337,7 @@ int eval(const Eval &e, const Layout &L, char *scratch, double *record, cudaStre
 extern "C" int b200_constant_scratch_bytes(int m, int n, int64_t *bytes) {
     B200_REQUIRE(m >= 0 && n >= 0 && bytes != nullptr, "bad arguments");
     B200_REQUIRE((int64_t)m * n <= (int64_t)1 << 30, "constant: frames of more than 2^30 pixels are not supported");
-    *bytes = (int64_t)layout(m, n).bytes;
+    *bytes = layout(m, n, nullptr).bytes;
     return 0;
 }
 
@@ -376,11 +346,11 @@ extern "C" int b200_constant_eval(const void *prev, const void *next, int dtype,
     B200_REQUIRE(m >= 0 && n >= 0 && scratch != nullptr && record != nullptr, "bad arguments");
     B200_REQUIRE((int64_t)m * n <= (int64_t)1 << 30, "constant: frames of more than 2^30 pixels are not supported");
     B200_REQUIRE((int64_t)m * n == 0 || (prev != nullptr && next != nullptr), "bad arguments");
-    const Layout L = layout(m, n);
+    const Layout L = layout(m, n, (char *)scratch);
     const Eval e{prev, next, m, n, vx, vy};
     cudaStream_t s = (cudaStream_t)stream;
-    if (dtype == B200_F32) return eval<float>(e, L, (char *)scratch, record, s);
-    if (dtype == B200_F64) return eval<double>(e, L, (char *)scratch, record, s);
+    if (dtype == B200_F32) return eval<float>(e, L, record, s);
+    if (dtype == B200_F64) return eval<double>(e, L, record, s);
     b200::set_error("constant: dtype must be B200_F32 or B200_F64");
     return B200_EINVAL;
 }

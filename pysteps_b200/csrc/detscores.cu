@@ -149,15 +149,12 @@ bool float_code(int c) { return c == B200_F32 || c == B200_F64; }
 // ---------------------------------------------------------------------------------------------------
 // moments
 
-template <typename P, typename Q> struct Promote { using T = double; };
-template <> struct Promote<float, float> { using T = float; };
-
 constexpr int NSUM = 9;
 constexpr int MOM_THREADS = 128;  // the per-element kernels hold nine sums and ten counts  // obs, pred, res, res^2, sum^2, |res|; cov, |obs - mobs|^2, |pred - mpred|^2
 
 template <typename P, typename Q>
 struct Mom {
-    using R = typename Promote<P, Q>::T;
+    using R = typename b200::Promote<P, Q>::T;
     const P *pred;
     const Q *obs;
     int cond;  // 0: all pairs, 1: pred > thr or obs > thr, 2: both

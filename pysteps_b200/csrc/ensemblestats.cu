@@ -15,6 +15,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "scan.cuh"
 
 namespace {
 
@@ -22,7 +23,6 @@ constexpr int THREADS = 256;
 constexpr int EXC_CHUNK = 8;        // thresholds counted per pass over X
 constexpr int MASK_THREADS = 1024;  // pixels per block of the mask scan
 constexpr int SCAN_THREADS = 1024;
-static_assert(MASK_THREADS == 1024 && SCAN_THREADS == 1024, "block_inclusive_scan assumes 32 warps");
 
 __device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
 __device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
@@ -30,8 +30,6 @@ __device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, 
 __device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
 __device__ __forceinline__ float to_f(double v, float) { return __double2float_rn(v); }
 __device__ __forceinline__ double to_f(double v, double) { return v; }
-
-__device__ __forceinline__ double quiet_nan() { return __longlong_as_double(0x7ff8000000000000ll); }
 
 // OR of v over the warp, then one integer atomic per warp that has a bit to report
 __device__ __forceinline__ void report(int v, int *flags) {
@@ -99,7 +97,7 @@ __global__ void __launch_bounds__(THREADS)
         if (ignore_nan && finite == 0) fl |= B200_ENSEMBLE_EMPTY;
 #pragma unroll
         for (int c = 0; c < EXC_CHUNK; c++)
-            if (c < th.count) out[c * N + pix] = nan_out ? quiet_nan() : __ddiv_rn((double)cnt[c], den);
+            if (c < th.count) out[c * N + pix] = nan_out ? b200::quiet_nan() : __ddiv_rn((double)cnt[c], den);
     }
     report(fl, flags);
 }
@@ -125,46 +123,11 @@ __global__ void __launch_bounds__(MASK_THREADS)
     if (threadIdx.x == 0) block_count[blockIdx.x] = c;
 }
 
-// inclusive sum of v over the block; sh: SCAN_THREADS / 32 words
-__device__ __forceinline__ int64_t block_inclusive_scan(int64_t v, int64_t *sh) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (int o = 1; o < 32; o <<= 1) {
-        const int64_t y = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += y;
-    }
-    if (lane == 31) sh[w] = v;
-    __syncthreads();
-    if (w == 0) {
-        int64_t s = sh[lane];
-        for (int o = 1; o < 32; o <<= 1) {
-            const int64_t y = __shfl_up_sync(0xffffffffu, s, o);
-            if (lane >= o) s += y;
-        }
-        sh[lane] = s;
-    }
-    __syncthreads();
-    const int64_t r = v + (w ? sh[w - 1] : 0);
-    __syncthreads();  // sh is reused by the next chunk
-    return r;
-}
-
 // one block: offset[b] = sum of block_count[0..b), offset[nblocks] = p
 __global__ void __launch_bounds__(SCAN_THREADS)
     band_offsets_kernel(const int *__restrict__ block_count, int nblocks, int64_t *__restrict__ offset) {
-    __shared__ int64_t sh[SCAN_THREADS / 32];
-    __shared__ int64_t total;
-    int64_t carry = 0;
-    for (int base = 0; base < nblocks; base += SCAN_THREADS) {
-        const int b = base + threadIdx.x;
-        const int64_t v = b < nblocks ? block_count[b] : 0;
-        const int64_t inc = block_inclusive_scan(v, sh);
-        if (b < nblocks) offset[b] = carry + inc - v;
-        if (threadIdx.x == SCAN_THREADS - 1) total = inc;
-        __syncthreads();
-        carry += total;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) offset[nblocks] = carry;
+    const int64_t p = b200::single_cta_scan<SCAN_THREADS>(block_count, nblocks, offset);
+    if (threadIdx.x == 0) offset[nblocks] = p;
 }
 
 // col[pix] = the pixel's column among the masked pixels in C order, -1 where it is not masked
@@ -174,8 +137,9 @@ __global__ void __launch_bounds__(MASK_THREADS)
     __shared__ int64_t sh[MASK_THREADS / 32];
     const int64_t pix = (int64_t)blockIdx.x * MASK_THREADS + threadIdx.x;
     const int64_t in = pix < N ? mask[pix] : 0;
-    const int64_t inc = block_inclusive_scan(in, sh);
-    if (pix < N) col[pix] = in ? (int)(offset[blockIdx.x] + inc - 1) : -1;
+    int64_t total;
+    const int64_t excl = b200::block_exclusive_scan<MASK_THREADS>(in, sh, &total);
+    if (pix < N) col[pix] = in ? (int)(offset[blockIdx.x] + excl) : -1;
 }
 
 // every member's rank at every masked pixel, 1 + #{j : (X_j, b_j) < (X_i, b_i)}, ties of both keys

@@ -21,14 +21,7 @@ namespace {
 
 constexpr int TX = 32, TY = 8;
 
-__device__ __forceinline__ int reflect101(int i, int L) {
-    if (L == 1) return 0;
-    while (i < 0 || i >= L) {
-        if (i < 0) i = -i;
-        if (i >= L) i = 2 * L - 2 - i;
-    }
-    return i;
-}
+using b200::reflect101;
 
 // mask = user_mask | !isfinite(img) (np.ma.masked_invalid); min/max over unmasked.
 // A pure stream over the frame (8 B read + 1 B written per pixel): PAIR = two pixels per thread as one

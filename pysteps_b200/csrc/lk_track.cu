@@ -37,14 +37,7 @@ struct LKParams {
     uint8_t *status;        // (npts)
 };
 
-__device__ __forceinline__ int reflect101(int i, int L) {
-    if (L == 1) return 0;
-    while (i < 0 || i >= L) {
-        if (i < 0) i = -i;
-        if (i >= L) i = 2 * L - 2 - i;
-    }
-    return i;
-}
+using b200::reflect101;
 
 __device__ __forceinline__ int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
 

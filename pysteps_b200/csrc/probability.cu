@@ -8,39 +8,13 @@
 //           overlaps the frame, then count / valid in float64, clipped to [0, 1]; NaN at NaN pixels
 // The sums are integers in a fixed order, so the result is the exact one, the same on every call.
 #include "common.cuh"
+#include "scan.cuh"
 
 namespace {
 
 constexpr int PREFIX_THREADS = 256, PREFIX_PER_THREAD = 4, PREFIX_TILE = PREFIX_THREADS * PREFIX_PER_THREAD;
 constexpr int RATIO_X = 32, RATIO_Y = 8;
 constexpr unsigned long long VALID_ONE = 1ull << 32;
-
-// exclusive prefix of v over the CTA; *total = the CTA's sum.  sh: THREADS / 32 words of shared memory
-template <int THREADS>
-__device__ __forceinline__ unsigned long long block_exclusive_scan(unsigned long long v, unsigned long long *sh,
-                                                                   unsigned long long *total) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned long long x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) sh[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        unsigned long long s = lane < THREADS / 32 ? sh[lane] : 0ull;
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, s, o);
-            if (lane >= o) s += y;
-        }
-        if (lane < THREADS / 32) sh[lane] = s;
-    }
-    __syncthreads();
-    const unsigned long long before = w ? sh[w - 1] : 0ull;
-    *total = sh[THREADS / 32 - 1];
-    __syncthreads();  // sh is reused by the next tile
-    return before + x - v;
-}
 
 // NaN pixels hold `threshold - 1` in the reference and exceed when that value does (nan_word); every
 // other pixel is valid and exceeds when (double)v >= threshold, the comparison NumPy makes in the
@@ -69,7 +43,7 @@ __global__ void __launch_bounds__(PREFIX_THREADS)
             sum += w[k];
         }
         unsigned long long total;
-        unsigned long long run = carry + block_exclusive_scan<PREFIX_THREADS>(sum, sh, &total);
+        unsigned long long run = carry + b200::block_exclusive_scan<PREFIX_THREADS>(sum, sh, &total);
 #pragma unroll
         for (int k = 0; k < PREFIX_PER_THREAD; k++) {
             if (x0 + k < n) out[x0 + k] = run;

@@ -1,5 +1,6 @@
-// radix_sort.cuh -- the stable LSD radix sort of (64-bit key, 32-bit index) pairs and the three-kernel
-// scan shared by salient blending (blending.cu) and probability matching (probmatching.cu), sm_90a.
+// radix_sort.cuh -- the stable LSD radix sort of (64-bit key, 32-bit index) pairs and a three-kernel
+// scan on the block scans of scan.cuh, shared by salient blending (blending.cu) and probability
+// matching (probmatching.cu), sm_90a.
 //   keys       order_key: an order-preserving 64-bit image of a double, -0.0 equal to +0.0
 //   sort       8-bit digits, least significant first; one global histogram of all eight digits
 //              plans the passes, and a digit that every key shares is skipped (plan_passes).  Each
@@ -11,8 +12,12 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "scan.cuh"
 
 namespace {
+
+using b200::Carver;
+using b200::quiet_nan;
 
 constexpr int THREADS = 256;
 constexpr int SORT_ITEMS = 16;
@@ -20,8 +25,6 @@ constexpr int TILE = THREADS * SORT_ITEMS;  // keys per radix tile and per scan 
 constexpr int RADIX = 256;
 constexpr int PASSES = 8;
 constexpr unsigned FULL = 0xffffffffu;
-
-__device__ __forceinline__ double quiet_nan() { return __longlong_as_double(0x7ff8000000000000ll); }
 
 // order-preserving 64-bit image of a double; -0.0 maps to +0.0 (rankdata treats them as equal)
 __device__ __forceinline__ unsigned long long order_key(double d) {
@@ -41,19 +44,6 @@ struct SortBuffers {
     unsigned *bsum;   // per scan block sums (also large enough for a scan over n values)
     unsigned *ghist;  // PASSES x RADIX global digit counts
     int *src;         // PASSES + 1: buffer each pass reads (-1: pass skipped); [PASSES]: the final buffer
-};
-
-static int64_t align256(int64_t b) { return (b + 255) & ~(int64_t)255; }
-
-// consecutive 256-byte aligned pieces of one scratch allocation; base == nullptr only sizes them
-struct Carver {
-    char *base;
-    int64_t off = 0;
-    void *take(int64_t bytes) {
-        char *p = base ? base + off : nullptr;
-        off += align256(bytes);
-        return p;
-    }
 };
 
 static void carve_sort(SortBuffers *s, Carver &c, int64_t n) {
@@ -115,32 +105,6 @@ __global__ void __launch_bounds__(THREADS)
     s.tiles[(int64_t)threadIdx.x * n_tiles + blockIdx.x] = h[threadIdx.x];
 }
 
-// block-wide exclusive scan of one value per thread; returns the total in *total
-__device__ __forceinline__ unsigned block_exclusive(unsigned v, unsigned *total) {
-    __shared__ unsigned warp_sum[THREADS / 32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned x = v;
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned y = __shfl_up_sync(FULL, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) warp_sum[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        unsigned s = lane < THREADS / 32 ? warp_sum[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned y = __shfl_up_sync(FULL, s, o);
-            if (lane >= o) s += y;
-        }
-        if (lane < THREADS / 32) warp_sum[lane] = s;
-    }
-    __syncthreads();
-    const unsigned before = (w ? warp_sum[w - 1] : 0) + x - v;
-    *total = warp_sum[THREADS / 32 - 1];
-    __syncthreads();
-    return before;
-}
-
 // the scan over the tile counts of a pass (exclusive, in place)
 struct CountScan {
     SortBuffers s;
@@ -155,32 +119,26 @@ struct CountScan {
 template <typename Op>
 __global__ void __launch_bounds__(THREADS) scan_reduce(Op op, int64_t n, unsigned *__restrict__ bsum) {
     if (op.skip()) return;
+    __shared__ unsigned sh[THREADS / 32];
     const int64_t i0 = (int64_t)blockIdx.x * TILE + (int64_t)threadIdx.x * SORT_ITEMS;
     unsigned v = 0;
     for (int r = 0; r < SORT_ITEMS; r++)
         if (i0 + r < n) v += op.load(i0 + r);
     unsigned total;
-    block_exclusive(v, &total);
+    b200::block_exclusive_scan<THREADS>(v, sh, &total);
     if (threadIdx.x == 0) bsum[blockIdx.x] = total;
 }
 
 template <typename Op>
 __global__ void __launch_bounds__(THREADS) scan_blocks(Op op, int64_t nb, unsigned *__restrict__ bsum) {
     if (op.skip()) return;
-    unsigned carry = 0;
-    for (int64_t b0 = 0; b0 < nb; b0 += THREADS) {
-        const int64_t b = b0 + threadIdx.x;
-        const unsigned v = b < nb ? bsum[b] : 0;
-        unsigned total;
-        const unsigned e = block_exclusive(v, &total);
-        if (b < nb) bsum[b] = carry + e;
-        carry += total;
-    }
+    b200::single_cta_scan<THREADS>(bsum, nb, bsum);
 }
 
 template <typename Op>
 __global__ void __launch_bounds__(THREADS) scan_apply(Op op, int64_t n, const unsigned *__restrict__ bsum) {
     if (op.skip()) return;
+    __shared__ unsigned sh[THREADS / 32];
     const int64_t i0 = (int64_t)blockIdx.x * TILE + (int64_t)threadIdx.x * SORT_ITEMS;
     unsigned v[SORT_ITEMS];
     unsigned sum = 0;
@@ -190,7 +148,7 @@ __global__ void __launch_bounds__(THREADS) scan_apply(Op op, int64_t n, const un
         sum += v[r];
     }
     unsigned total;
-    unsigned run = bsum[blockIdx.x] + block_exclusive(sum, &total);
+    unsigned run = bsum[blockIdx.x] + b200::block_exclusive_scan<THREADS>(sum, sh, &total);
 #pragma unroll
     for (int r = 0; r < SORT_ITEMS; r++) {
         if (i0 + r < n) op.store(i0 + r, run, v[r]);

@@ -22,15 +22,12 @@
 
 #include "common.cuh"
 #include "pairwise_body.cuh"
+#include "scan.cuh"
 
 namespace {
 
 constexpr int THREADS = 256;
 constexpr int SCAN_THREADS = 1024;
-
-// the dtype NumPy computes a difference of an F and an O in
-template <typename F, typename O> struct Promote { using T = double; };
-template <> struct Promote<float, float> { using T = float; };
 
 __device__ __forceinline__ bool finite(double v) { return isfinite(v); }
 
@@ -63,51 +60,15 @@ __global__ void __launch_bounds__(THREADS)
     for (int i = threadIdx.x; i < nkeys; i += THREADS) counts[(int64_t)i * gridDim.x + blockIdx.x] = hist[i];
 }
 
-// inclusive sum of v over the block; sh: SCAN_THREADS / 32 words
-__device__ __forceinline__ int64_t block_inclusive_scan(int64_t v, int64_t *sh) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (int o = 1; o < 32; o <<= 1) {
-        const int64_t y = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += y;
-    }
-    if (lane == 31) sh[w] = v;
-    __syncthreads();
-    if (w == 0) {
-        int64_t s = sh[lane];
-        for (int o = 1; o < 32; o <<= 1) {
-            const int64_t y = __shfl_up_sync(0xffffffffu, s, o);
-            if (lane >= o) s += y;
-        }
-        sh[lane] = s;
-    }
-    __syncthreads();
-    const int64_t r = v + (w ? sh[w - 1] : 0);
-    __syncthreads();
-    return r;
-}
-
 // one block: offset[i] = the exclusive sum of counts[0..i); seg[key] = offset[key * blocks],
 // seg[nkeys] = the total
 __global__ void __launch_bounds__(SCAN_THREADS)
     part_scan_kernel(const int *__restrict__ counts, int64_t n, int blocks, int nkeys, int64_t *__restrict__ offset,
                      int64_t *__restrict__ seg) {
-    __shared__ int64_t sh[SCAN_THREADS / 32];
-    __shared__ int64_t total;
-    int64_t carry = 0;
-    for (int64_t base = 0; base < n; base += SCAN_THREADS) {
-        const int64_t i = base + threadIdx.x;
-        const int64_t v = i < n ? counts[i] : 0;
-        const int64_t inc = block_inclusive_scan(v, sh);
-        if (i < n) {
-            offset[i] = carry + inc - v;
-            if (i % blocks == 0) seg[i / blocks] = carry + inc - v;
-        }
-        if (threadIdx.x == SCAN_THREADS - 1) total = inc;
-        __syncthreads();
-        carry += total;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) seg[nkeys] = carry;
+    const int64_t total = b200::single_cta_scan<SCAN_THREADS>(counts, n, offset);
+    __syncthreads();  // seg is read from offsets that other threads wrote
+    for (int key = threadIdx.x; key < nkeys; key += SCAN_THREADS) seg[key] = offset[(int64_t)key * blocks];
+    if (threadIdx.x == 0) seg[nkeys] = total;
 }
 
 // out[offset of (key, block) + the pixel's rank among the earlier pixels of its key] = val[pix]
@@ -269,7 +230,7 @@ template <typename F, typename O, typename Members>
 __global__ void __launch_bounds__(THREADS)
     crps_kernel(const F *__restrict__ X, const O *__restrict__ obs, int k, int64_t N, F *scratch,
                 double *__restrict__ res, int *__restrict__ key) {
-    using P = typename Promote<F, O>::T;
+    using P = typename b200::Promote<F, O>::T;
     const int64_t pix = (int64_t)blockIdx.x * THREADS + threadIdx.x;
     if (pix >= N) return;
     const O o = obs[pix];
