@@ -31,6 +31,9 @@
 extern "C" {
 #endif
 
+/* Field dtype codes.  An entry point refuses any other code with B200_EINVAL, and names it in
+ * b200_last_error(), before it does any device work (allocation, memset, copy or launch) and
+ * before it returns early on empty input. */
 #define B200_F32 0
 #define B200_F64 1
 
@@ -196,9 +199,6 @@ int b200_sl_extrapolate_host(const void *precip, const void *velocity,
 int b200_field_stats(const void *a, int field_dtype, int64_t count, double *stats,
                      void *stream);
 
-/* dtype conversion on device (float64 <-> float32), count elements */
-int b200_convert(const void *src, int src_dtype, void *dst, int dst_dtype,
-                 int64_t count, void *stream);
 /* dst[0..count) = value (float64) */
 int b200_fill_f64(double *dst, int64_t count, double value, void *stream);
 

@@ -125,7 +125,6 @@ _SIGNATURES = {
                                   c_void_p, c_void_p, c_void_p]),
     "b200_darts_synthesize": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
                                       c_void_p]),
-    "b200_convert":(c_int, [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p]),
     "b200_probability": (c_int, [c_void_p, c_int, c_i64, c_int, c_int, c_int, c_double, c_int,
                                  ctypes.POINTER(c_int), c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200_ensemble_mean": (c_int, [c_void_p, c_int, c_int, c_i64, c_int, c_int, c_double, c_void_p, c_void_p,

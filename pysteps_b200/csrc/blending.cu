@@ -328,49 +328,41 @@ extern "C" int b200_blend_transform(const void *x, void *y, int dtype, int64_t n
                      (kind < B200_BLEND_DB || nfix != nullptr),
                  "bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
-    if (nfix) B200_CUDA(cudaMemsetAsync(nfix, 0, sizeof(unsigned long long), st));
-    if (n == 0) return 0;
-    B200_REQUIRE(x != nullptr && y != nullptr && (cap == 0 || (fix_idx != nullptr && fix_x != nullptr)),
-                 "bad arguments");
-    if (dtype == B200_F32) return transform_run<float>(x, y, n, kind, lam, thr, zero, fix_idx, fix_x, cap, nfix, st);
-    if (dtype == B200_F64) return transform_run<double>(x, y, n, kind, lam, thr, zero, fix_idx, fix_x, cap, nfix, st);
-    b200::set_error("blend_transform: dtype must be B200_F32 or B200_F64");
-    return B200_EINVAL;
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        if (nfix) B200_CUDA(cudaMemsetAsync(nfix, 0, sizeof(unsigned long long), st));
+        if (n == 0) return 0;
+        B200_REQUIRE(x != nullptr && y != nullptr && (cap == 0 || (fix_idx != nullptr && fix_x != nullptr)),
+                     "bad arguments");
+        return transform_run<F>(x, y, n, kind, lam, thr, zero, fix_idx, fix_x, cap, nfix, st);
+    });
 }
 
 extern "C" int b200_blend_unit(const void *x, void *y, int dtype, int64_t n, int kind, double a, double b,
                                void *stream) {
     B200_REQUIRE(n >= 0 && (kind == B200_BLEND_MM || kind == B200_BLEND_DBZ), "bad arguments");
-    if (n == 0) return 0;
-    B200_REQUIRE(x != nullptr && y != nullptr, "bad arguments");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == B200_F32)
-        unit_kernel<float><<<grid_for(n), THREADS, 0, st>>>((const float *)x, (float *)y, n, kind, a, b);
-    else if (dtype == B200_F64)
-        unit_kernel<double><<<grid_for(n), THREADS, 0, st>>>((const double *)x, (double *)y, n, kind, a, b);
-    else {
-        b200::set_error("blend_unit: dtype must be B200_F32 or B200_F64");
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
-    return 0;
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        if (n == 0) return 0;
+        B200_REQUIRE(x != nullptr && y != nullptr, "bad arguments");
+        unit_kernel<F><<<grid_for(n), THREADS, 0, (cudaStream_t)stream>>>((const F *)x, (F *)y, n, kind, a, b);
+        B200_LAUNCH_CHECK();
+        return 0;
+    });
 }
 
 extern "C" int b200_blend_scatter(void *y, int dtype, const long long *idx, const double *val, int64_t n,
                                   void *stream) {
     B200_REQUIRE(n >= 0, "bad arguments");
-    if (n == 0) return 0;
-    B200_REQUIRE(y != nullptr && idx != nullptr && val != nullptr, "bad arguments");
-    cudaStream_t st = (cudaStream_t)stream;
-    const unsigned g = (unsigned)b200::ceil_div64(n, THREADS);
-    if (dtype == B200_F32) scatter_kernel<float><<<g, THREADS, 0, st>>>((float *)y, idx, val, n);
-    else if (dtype == B200_F64) scatter_kernel<double><<<g, THREADS, 0, st>>>((double *)y, idx, val, n);
-    else {
-        b200::set_error("blend_scatter: dtype must be B200_F32 or B200_F64");
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
-    return 0;
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        if (n == 0) return 0;
+        B200_REQUIRE(y != nullptr && idx != nullptr && val != nullptr, "bad arguments");
+        const unsigned g = (unsigned)b200::ceil_div64(n, THREADS);
+        scatter_kernel<F><<<g, THREADS, 0, (cudaStream_t)stream>>>((F *)y, idx, val, n);
+        B200_LAUNCH_CHECK();
+        return 0;
+    });
 }
 
 static bool fields_ok(const void *now, const int *now_map, const void *nwp, const int *nwp_map, const void *out) {
@@ -382,18 +374,15 @@ extern "C" int b200_blend_linear(const void *now, int now_dtype, const int *now_
                                  int n_out, int T, int64_t P, const int *mode, const int *bits, const double *w_nwp,
                                  const double *w_now, int fill_nwp, void *stream) {
     B200_REQUIRE(n_out >= 0 && T >= 0 && P >= 0 && (int64_t)n_out * T <= INT32_MAX, "bad arguments");
-    if ((int64_t)n_out * T * P == 0) return 0;
-    // now may be NULL when the nowcast has no lead (every lead is then B200_BLEND_NWP)
-    B200_REQUIRE(now_map && nwp && nwp_map && out && mode && bits && w_nwp && w_now, "bad arguments");
-    const Fields f{now, now_map, now_member, nwp, nwp_map, nwp_member, P, fill_nwp};
-    cudaStream_t st = (cudaStream_t)stream;
-    const int c = now_dtype * 2 + nwp_dtype;
-    if (c == 0) return linear_run<float, float>(f, out, n_out, T, mode, bits, w_nwp, w_now, st);
-    if (c == 1) return linear_run<float, double>(f, out, n_out, T, mode, bits, w_nwp, w_now, st);
-    if (c == 2) return linear_run<double, float>(f, out, n_out, T, mode, bits, w_nwp, w_now, st);
-    if (c == 3) return linear_run<double, double>(f, out, n_out, T, mode, bits, w_nwp, w_now, st);
-    b200::set_error("blend_linear: dtypes must be B200_F32 or B200_F64");
-    return B200_EINVAL;
+    return b200::with_dtypes(now_dtype, nwp_dtype, [&](auto tc, auto tn) {
+        using Tc = typename decltype(tc)::type;
+        using Tn = typename decltype(tn)::type;
+        if ((int64_t)n_out * T * P == 0) return 0;
+        // now may be NULL when the nowcast has no lead (every lead is then B200_BLEND_NWP)
+        B200_REQUIRE(now_map && nwp && nwp_map && out && mode && bits && w_nwp && w_now, "bad arguments");
+        const Fields f{now, now_map, now_member, nwp, nwp_map, nwp_member, P, fill_nwp};
+        return linear_run<Tc, Tn>(f, out, n_out, T, mode, bits, w_nwp, w_now, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200_blend_salient(const void *now, int now_dtype, const int *now_map, int64_t now_member,
@@ -402,41 +391,37 @@ extern "C" int b200_blend_salient(const void *now, int now_dtype, const int *now
                                   int fill_nwp, void *scratch, int64_t scratch_bytes, void *stream) {
     const int64_t n = (int64_t)n_out * P;
     B200_REQUIRE(n_out >= 0 && P >= 0 && n < ((int64_t)1 << 31) && lead >= 0 && lead < T, "bad arguments");
-    if (n == 0) return 0;
-    SortScratch s;
-    B200_REQUIRE(fields_ok(now, now_map, nwp, nwp_map, out) && scratch && scratch_bytes >= carve(&s, nullptr, n),
-                 "bad arguments");
-    const Fields f{now, now_map, now_member, nwp, nwp_map, nwp_member, P, fill_nwp};
-    cudaStream_t st = (cudaStream_t)stream;
-    const int c = now_dtype * 2 + nwp_dtype;
-    if (c == 0) return salient_run<float, float, float>(f, out, n_out, T, lead, w, w1, w2, w12, scratch, st);
-    if (c == 1) return salient_run<float, double, double>(f, out, n_out, T, lead, w, w1, w2, w12, scratch, st);
-    if (c == 2) return salient_run<double, float, double>(f, out, n_out, T, lead, w, w1, w2, w12, scratch, st);
-    if (c == 3) return salient_run<double, double, double>(f, out, n_out, T, lead, w, w1, w2, w12, scratch, st);
-    b200::set_error("blend_salient: dtypes must be B200_F32 or B200_F64");
-    return B200_EINVAL;
+    return b200::with_dtypes(now_dtype, nwp_dtype, [&](auto tc, auto tn) {
+        using Tc = typename decltype(tc)::type;
+        using Tn = typename decltype(tn)::type;
+        if (n == 0) return 0;
+        SortScratch s;
+        B200_REQUIRE(fields_ok(now, now_map, nwp, nwp_map, out) && scratch && scratch_bytes >= carve(&s, nullptr, n),
+                     "bad arguments");
+        const Fields f{now, now_map, now_member, nwp, nwp_map, nwp_member, P, fill_nwp};
+        return salient_run<Tc, Tn, typename b200::Promote<Tc, Tn>::T>(f, out, n_out, T, lead, w, w1, w2, w12, scratch,
+                                                                      (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200_dense_rank(const void *x, int dtype, int64_t n, unsigned *rank, unsigned *max_rank, int *nan_flag,
                                void *scratch, int64_t scratch_bytes, void *stream) {
     B200_REQUIRE(n >= 0 && n < ((int64_t)1 << 31), "bad arguments");
-    if (n == 0) return 0;
-    SortScratch s;
-    B200_REQUIRE(x && rank && max_rank && nan_flag && scratch && scratch_bytes >= carve(&s, nullptr, n),
-                 "bad arguments");
-    carve(&s, (char *)scratch, n);
-    cudaStream_t st = (cudaStream_t)stream;
-    B200_CUDA(cudaMemsetAsync(s.nan_flag, 0, 4, st));
-    if (dtype == B200_F32) array_keys<float><<<grid_for(n), THREADS, 0, st>>>((const float *)x, n, s.sort.key[0], s.sort.idx[0], s.nan_flag);
-    else if (dtype == B200_F64) array_keys<double><<<grid_for(n), THREADS, 0, st>>>((const double *)x, n, s.sort.key[0], s.sort.idx[0], s.nan_flag);
-    else {
-        b200::set_error("dense_rank: dtype must be B200_F32 or B200_F64");
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
-    if (int rc = dense_rank(s, n, st)) return rc;
-    B200_CUDA(cudaMemcpyAsync(rank, s.rank, 4 * n, cudaMemcpyDeviceToDevice, st));
-    B200_CUDA(cudaMemcpyAsync(max_rank, s.max_rank, 4, cudaMemcpyDeviceToDevice, st));
-    B200_CUDA(cudaMemcpyAsync(nan_flag, s.nan_flag, 4, cudaMemcpyDeviceToDevice, st));
-    return 0;
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        if (n == 0) return 0;
+        SortScratch s;
+        B200_REQUIRE(x && rank && max_rank && nan_flag && scratch && scratch_bytes >= carve(&s, nullptr, n),
+                     "bad arguments");
+        carve(&s, (char *)scratch, n);
+        cudaStream_t st = (cudaStream_t)stream;
+        B200_CUDA(cudaMemsetAsync(s.nan_flag, 0, 4, st));
+        array_keys<F><<<grid_for(n), THREADS, 0, st>>>((const F *)x, n, s.sort.key[0], s.sort.idx[0], s.nan_flag);
+        B200_LAUNCH_CHECK();
+        if (int rc = dense_rank(s, n, st)) return rc;
+        B200_CUDA(cudaMemcpyAsync(rank, s.rank, 4 * n, cudaMemcpyDeviceToDevice, st));
+        B200_CUDA(cudaMemcpyAsync(max_rank, s.max_rank, 4, cudaMemcpyDeviceToDevice, st));
+        B200_CUDA(cudaMemcpyAsync(nan_flag, s.nan_flag, 4, cudaMemcpyDeviceToDevice, st));
+        return 0;
+    });
 }

@@ -38,6 +38,27 @@ void count_launch();
         }                                                                  \
     } while (0)
 
+template <typename T> struct Type { using type = T; };
+
+// f(Type<float>{}) or f(Type<double>{}) for a dtype code; any other code is refused, named as the dtype of `what`
+template <typename Fn>
+int with_dtype(const char *what, int dtype, Fn &&f) {
+    if (dtype == B200_F32) return f(Type<float>{});
+    if (dtype == B200_F64) return f(Type<double>{});
+    set_error("unknown %s dtype %d", what, dtype);
+    return B200_EINVAL;
+}
+
+// f(Type<A>{}, Type<B>{}) for the dtype codes of two fields, refused before f runs when either code is unknown
+template <typename Fn>
+int with_dtypes(int a, int b, Fn &&f) {
+    if ((a != B200_F32 && a != B200_F64) || (b != B200_F32 && b != B200_F64)) {
+        set_error("unknown field dtypes %d / %d", a, b);
+        return B200_EINVAL;
+    }
+    return with_dtype("field", a, [&](auto ta) { return with_dtype("field", b, [&](auto tb) { return f(ta, tb); }); });
+}
+
 // stream-ordered scratch allocation that is released on scope exit
 struct Scratch {
     void *p = nullptr;

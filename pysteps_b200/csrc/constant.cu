@@ -349,8 +349,5 @@ extern "C" int b200_constant_eval(const void *prev, const void *next, int dtype,
     const Layout L = layout(m, n, (char *)scratch);
     const Eval e{prev, next, m, n, vx, vy};
     cudaStream_t s = (cudaStream_t)stream;
-    if (dtype == B200_F32) return eval<float>(e, L, record, s);
-    if (dtype == B200_F64) return eval<double>(e, L, record, s);
-    b200::set_error("constant: dtype must be B200_F32 or B200_F64");
-    return B200_EINVAL;
+    return b200::with_dtype("frame", dtype, [&](auto t) { return eval<typename decltype(t)::type>(e, L, record, s); });
 }

@@ -308,10 +308,10 @@ extern "C" int b200_darts_spectrum(const void *frames, int dtype, int T, int m, 
     cudaStream_t s = (cudaStream_t)stream;
     const double2 *tx = (const double2 *)tw_x, *ty = (const double2 *)tw_y, *tt = (const double2 *)tw_t;
     double2 *w = (double2 *)work, *X = (double2 *)spectrum_out;
-    if (dtype == B200_F32) return spectrum<float>((const float *)frames, T, m, n, tx, fx, ty, Ky, tt, Kt, K, w, X, s);
-    if (dtype == B200_F64) return spectrum<double>((const double *)frames, T, m, n, tx, fx, ty, Ky, tt, Kt, K, w, X, s);
-    b200::set_error("darts: dtype must be B200_F32 or B200_F64");
-    return B200_EINVAL;
+    return b200::with_dtype("frame", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        return spectrum<F>((const F *)frames, T, m, n, tx, fx, ty, Ky, tt, Kt, K, w, X, s);
+    });
 }
 
 extern "C" int b200_darts_normal(const double *spectrum_in, int N_x, int N_y, int N_t, int M_x, int M_y, double sx,

@@ -144,8 +144,6 @@ int contab_run(const P *pred, const O *obs, double thr_p, double thr_o, const Ax
     return 0;
 }
 
-bool float_code(int c) { return c == B200_F32 || c == B200_F64; }
-
 // ---------------------------------------------------------------------------------------------------
 // moments
 
@@ -429,20 +427,18 @@ extern "C" int b200_verif_contab(const void *pred, int p_dtype, const void *obs,
                                  double thr_o, const int64_t *kept_size, const int64_t *kept_stride, int n_kept,
                                  const int64_t *red_size, const int64_t *red_stride, int n_red, int64_t *counts,
                                  void *stream) {
-    B200_REQUIRE(float_code(p_dtype) && float_code(o_dtype), "verif_contab: dtypes must be B200_F32 or B200_F64");
-    Axes kept, red;
-    if (int rc = axes_from(kept_size, kept_stride, n_kept, &kept)) return rc;
-    if (int rc = axes_from(red_size, red_stride, n_red, &red)) return rc;
-    const int64_t M = count_of(kept), R = count_of(red);
-    B200_REQUIRE(M * R < ((int64_t)1 << 31) && counts != nullptr && pred != nullptr && obs != nullptr,
-                 "verif_contab: bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-#define B200_RUN(P, O) contab_run<P, O>((const P *)pred, (const O *)obs, thr_p, thr_o, kept, red, M, R, counts, s)
-    if (p_dtype == B200_F32 && o_dtype == B200_F32) return B200_RUN(float, float);
-    if (p_dtype == B200_F32) return B200_RUN(float, double);
-    if (o_dtype == B200_F32) return B200_RUN(double, float);
-    return B200_RUN(double, double);
-#undef B200_RUN
+    return b200::with_dtypes(p_dtype, o_dtype, [&](auto tp, auto to) {
+        using P = typename decltype(tp)::type;
+        using O = typename decltype(to)::type;
+        Axes kept, red;
+        if (int rc = axes_from(kept_size, kept_stride, n_kept, &kept)) return rc;
+        if (int rc = axes_from(red_size, red_stride, n_red, &red)) return rc;
+        const int64_t M = count_of(kept), R = count_of(red);
+        B200_REQUIRE(M * R < ((int64_t)1 << 31) && counts != nullptr && pred != nullptr && obs != nullptr,
+                     "verif_contab: bad arguments");
+        return contab_run<P, O>((const P *)pred, (const O *)obs, thr_p, thr_o, kept, red, M, R, counts,
+                                (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200_verif_cont_moments(const void *pred, int p_dtype, const void *obs, int o_dtype, int conditioning,
@@ -450,23 +446,19 @@ extern "C" int b200_verif_cont_moments(const void *pred, int p_dtype, const void
                                        const int64_t *kept_stride, int n_kept, const int64_t *outer_size,
                                        const int64_t *outer_stride, int n_outer, int64_t L, double *tot,
                                        int64_t *cnt, int *infs, int *flags, void *stream) {
-    B200_REQUIRE(float_code(p_dtype) && float_code(o_dtype), "verif_cont_moments: dtypes must be B200_F32 or B200_F64");
-    B200_REQUIRE(conditioning >= 0 && conditioning <= 2 && L >= 1, "verif_cont_moments: bad arguments");
-    Axes kept, outer;
-    if (int rc = axes_from(kept_size, kept_stride, n_kept, &kept)) return rc;
-    if (int rc = axes_from(outer_size, outer_stride, n_outer, &outer)) return rc;
-    const int64_t M = count_of(kept), O = count_of(outer);
-    B200_REQUIRE(M * O * L < ((int64_t)1 << 31) && pred != nullptr && obs != nullptr && tot != nullptr &&
-                     cnt != nullptr && infs != nullptr && flags != nullptr,
-                 "verif_cont_moments: bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-#define B200_RUN(P, O_)                                                                                          \
-    moments_run<P, O_>(Mom<P, O_>{(const P *)pred, (const O_ *)obs, conditioning, thr_p, thr_o, kept, outer, M, O, L, \
-                                  1, 0, nullptr, tot, (long long *)cnt, infs, flags},                            \
-                       s)
-    if (p_dtype == B200_F32 && o_dtype == B200_F32) return B200_RUN(float, float);
-    if (p_dtype == B200_F32) return B200_RUN(float, double);
-    if (o_dtype == B200_F32) return B200_RUN(double, float);
-    return B200_RUN(double, double);
-#undef B200_RUN
+    return b200::with_dtypes(p_dtype, o_dtype, [&](auto tp, auto tq) {
+        using P = typename decltype(tp)::type;
+        using Q = typename decltype(tq)::type;
+        B200_REQUIRE(conditioning >= 0 && conditioning <= 2 && L >= 1, "verif_cont_moments: bad arguments");
+        Axes kept, outer;
+        if (int rc = axes_from(kept_size, kept_stride, n_kept, &kept)) return rc;
+        if (int rc = axes_from(outer_size, outer_stride, n_outer, &outer)) return rc;
+        const int64_t M = count_of(kept), O = count_of(outer);
+        B200_REQUIRE(M * O * L < ((int64_t)1 << 31) && pred != nullptr && obs != nullptr && tot != nullptr &&
+                         cnt != nullptr && infs != nullptr && flags != nullptr,
+                     "verif_cont_moments: bad arguments");
+        return moments_run<P, Q>(Mom<P, Q>{(const P *)pred, (const Q *)obs, conditioning, thr_p, thr_o, kept, outer, M,
+                                           O, L, 1, 0, nullptr, tot, (long long *)cnt, infs, flags},
+                                 (cudaStream_t)stream);
+    });
 }

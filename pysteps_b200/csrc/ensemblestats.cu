@@ -213,83 +213,77 @@ extern "C" int b200_ensemble_mean(const void *X, int dtype, int k, int64_t N, in
                                   void *out, int *flags, void *stream) {
     B200_REQUIRE(k >= 0 && N >= 0 && N < ((int64_t)1 << 31) && flags != nullptr, "bad arguments");
     cudaStream_t s = (cudaStream_t)stream;
-    B200_CUDA(cudaMemsetAsync(flags, 0, sizeof(int), s));
-    if (N == 0) return 0;
-    B200_REQUIRE(out != nullptr && (k == 0 || X != nullptr), "bad arguments");
-    if (dtype == B200_F32)
-        return mean_run<float>((const float *)X, k, N, nan_mode, use_thr, thr, (float *)out, flags, s);
-    if (dtype == B200_F64)
-        return mean_run<double>((const double *)X, k, N, nan_mode, use_thr, thr, (double *)out, flags, s);
-    b200::set_error("ensemble_mean: dtype must be B200_F32 or B200_F64");
-    return B200_EINVAL;
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        B200_CUDA(cudaMemsetAsync(flags, 0, sizeof(int), s));
+        if (N == 0) return 0;
+        B200_REQUIRE(out != nullptr && (k == 0 || X != nullptr), "bad arguments");
+        return mean_run<F>((const F *)X, k, N, nan_mode, use_thr, thr, (F *)out, flags, s);
+    });
 }
 
 extern "C" int b200_ensemble_excprob(const void *X, int dtype, int k, int64_t N, const double *thr, int n_thr,
                                      int ignore_nan, double *out, int *flags, void *stream) {
     B200_REQUIRE(k >= 0 && N >= 0 && N < ((int64_t)1 << 31) && n_thr >= 0 && flags != nullptr, "bad arguments");
     cudaStream_t s = (cudaStream_t)stream;
-    B200_CUDA(cudaMemsetAsync(flags, 0, sizeof(int), s));
-    if (N == 0 || n_thr == 0) return 0;
-    B200_REQUIRE(thr != nullptr && out != nullptr && (k == 0 || X != nullptr), "bad arguments");
-    if (dtype == B200_F32)
-        return excprob_run<float>((const float *)X, k, N, thr, n_thr, ignore_nan, out, flags, s);
-    if (dtype == B200_F64)
-        return excprob_run<double>((const double *)X, k, N, thr, n_thr, ignore_nan, out, flags, s);
-    b200::set_error("ensemble_excprob: dtype must be B200_F32 or B200_F64");
-    return B200_EINVAL;
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        B200_CUDA(cudaMemsetAsync(flags, 0, sizeof(int), s));
+        if (N == 0 || n_thr == 0) return 0;
+        B200_REQUIRE(thr != nullptr && out != nullptr && (k == 0 || X != nullptr), "bad arguments");
+        return excprob_run<F>((const F *)X, k, N, thr, n_thr, ignore_nan, out, flags, s);
+    });
 }
 
 extern "C" int b200_ensemble_band_mask(const void *X, int dtype, int k, int64_t N, double thr, int *col, int64_t *p,
                                        void *stream) {
     B200_REQUIRE(k >= 0 && N >= 0 && N < ((int64_t)1 << 31) && p != nullptr, "bad arguments");
-    B200_REQUIRE(dtype == B200_F32 || dtype == B200_F64, "ensemble_band_mask: dtype must be B200_F32 or B200_F64");
     cudaStream_t s = (cudaStream_t)stream;
-    if (N == 0) {
-        B200_CUDA(cudaMemsetAsync(p, 0, sizeof(int64_t), s));
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        if (N == 0) {
+            B200_CUDA(cudaMemsetAsync(p, 0, sizeof(int64_t), s));
+            return 0;
+        }
+        B200_REQUIRE(col != nullptr && (k == 0 || X != nullptr), "bad arguments");
+        const int nblocks = (int)b200::ceil_div64(N, MASK_THREADS);
+        b200::Scratch mask, counts, offsets;
+        B200_CUDA(mask.alloc((size_t)N, s));
+        B200_CUDA(counts.alloc(sizeof(int) * nblocks, s));
+        B200_CUDA(offsets.alloc(sizeof(int64_t) * (nblocks + 1), s));
+        unsigned char *m = (unsigned char *)mask.p;
+        band_mask_kernel<F><<<nblocks, MASK_THREADS, 0, s>>>((const F *)X, k, N, thr, m, (int *)counts.p);
+        B200_LAUNCH_CHECK();
+        int64_t *off = (int64_t *)offsets.p;
+        band_offsets_kernel<<<1, SCAN_THREADS, 0, s>>>((const int *)counts.p, nblocks, off);
+        B200_LAUNCH_CHECK();
+        band_columns_kernel<<<nblocks, MASK_THREADS, 0, s>>>(m, N, off, col);
+        B200_LAUNCH_CHECK();
+        B200_CUDA(cudaMemcpyAsync(p, off + nblocks, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
         return 0;
-    }
-    B200_REQUIRE(col != nullptr && (k == 0 || X != nullptr), "bad arguments");
-    const int nblocks = (int)b200::ceil_div64(N, MASK_THREADS);
-    b200::Scratch mask, counts, offsets;
-    B200_CUDA(mask.alloc((size_t)N, s));
-    B200_CUDA(counts.alloc(sizeof(int) * nblocks, s));
-    B200_CUDA(offsets.alloc(sizeof(int64_t) * (nblocks + 1), s));
-    unsigned char *m = (unsigned char *)mask.p;
-    if (dtype == B200_F32)
-        band_mask_kernel<float><<<nblocks, MASK_THREADS, 0, s>>>((const float *)X, k, N, thr, m, (int *)counts.p);
-    else
-        band_mask_kernel<double><<<nblocks, MASK_THREADS, 0, s>>>((const double *)X, k, N, thr, m, (int *)counts.p);
-    B200_LAUNCH_CHECK();
-    int64_t *off = (int64_t *)offsets.p;
-    band_offsets_kernel<<<1, SCAN_THREADS, 0, s>>>((const int *)counts.p, nblocks, off);
-    B200_LAUNCH_CHECK();
-    band_columns_kernel<<<nblocks, MASK_THREADS, 0, s>>>(m, N, off, col);
-    B200_LAUNCH_CHECK();
-    B200_CUDA(cudaMemcpyAsync(p, off + nblocks, sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
-    return 0;
+    });
 }
 
 extern "C" int b200_ensemble_band_match(const void *X, int dtype, int k, int64_t N, const int *col, const double *b,
                                         int64_t p, int64_t *match, void *stream) {
     B200_REQUIRE(k >= 0 && N >= 0 && N < ((int64_t)1 << 31) && p >= 0 && p <= N, "bad arguments");
-    B200_REQUIRE(dtype == B200_F32 || dtype == B200_F64, "ensemble_band_match: dtype must be B200_F32 or B200_F64");
-    if (k == 0) return 0;
-    B200_REQUIRE(match != nullptr, "bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-    B200_CUDA(cudaMemsetAsync(match, 0, sizeof(int64_t) * k, s));
-    if (p == 0) return 0;
-    B200_REQUIRE(X != nullptr && col != nullptr && b != nullptr, "bad arguments");
-    const int blocks = (int)std::min<int64_t>(b200::ceil_div64(N, THREADS), (int64_t)b200::num_sms() * 8);
-    b200::Scratch partial;
-    B200_CUDA(partial.alloc(sizeof(unsigned long long) * blocks * k, s));
-    B200_CUDA(cudaMemsetAsync(partial.p, 0, sizeof(unsigned long long) * blocks * k, s));
-    unsigned long long *part = (unsigned long long *)partial.p;
-    if (dtype == B200_F32)
-        band_match_kernel<float><<<blocks, THREADS, 0, s>>>((const float *)X, k, N, col, b, p, part);
-    else
-        band_match_kernel<double><<<blocks, THREADS, 0, s>>>((const double *)X, k, N, col, b, p, part);
-    B200_LAUNCH_CHECK();
-    band_sum_kernel<<<b200::ceil_div(k, THREADS), THREADS, 0, s>>>(part, blocks, k, match);
-    B200_LAUNCH_CHECK();
-    return 0;
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        if (k == 0) return 0;
+        B200_REQUIRE(match != nullptr, "bad arguments");
+        cudaStream_t s = (cudaStream_t)stream;
+        B200_CUDA(cudaMemsetAsync(match, 0, sizeof(int64_t) * k, s));
+        if (p == 0) return 0;
+        B200_REQUIRE(X != nullptr && col != nullptr && b != nullptr, "bad arguments");
+        const int blocks = (int)std::min<int64_t>(b200::ceil_div64(N, THREADS), (int64_t)b200::num_sms() * 8);
+        b200::Scratch partial;
+        B200_CUDA(partial.alloc(sizeof(unsigned long long) * blocks * k, s));
+        B200_CUDA(cudaMemsetAsync(partial.p, 0, sizeof(unsigned long long) * blocks * k, s));
+        unsigned long long *part = (unsigned long long *)partial.p;
+        band_match_kernel<F><<<blocks, THREADS, 0, s>>>((const F *)X, k, N, col, b, p, part);
+        B200_LAUNCH_CHECK();
+        band_sum_kernel<<<b200::ceil_div(k, THREADS), THREADS, 0, s>>>(part, blocks, k, match);
+        B200_LAUNCH_CHECK();
+        return 0;
+    });
 }

@@ -164,12 +164,12 @@ extern "C" int b200_fss_fractions(const void *X, int dtype, int nf, int m, int n
                                   double *S, void *stream) {
     B200_REQUIRE(nf >= 0 && m >= 0 && n >= 0 && s >= 0 && (int64_t)nf * m * n < ((int64_t)1 << 31),
                  "fss_fractions: bad arguments");
-    B200_REQUIRE(dtype == B200_F32 || dtype == B200_F64, "fss_fractions: dtype must be B200_F32 or B200_F64");
-    if ((int64_t)nf * m * n == 0) return 0;
-    B200_REQUIRE(X != nullptr && S != nullptr, "fss_fractions: bad arguments");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dtype == B200_F32) return fractions_run<float>((const float *)X, nf, m, n, thr, sub, s, S, st);
-    return fractions_run<double>((const double *)X, nf, m, n, thr, sub, s, S, st);
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        if ((int64_t)nf * m * n == 0) return 0;
+        B200_REQUIRE(X != nullptr && S != nullptr, "fss_fractions: bad arguments");
+        return fractions_run<F>((const F *)X, nf, m, n, thr, sub, s, S, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200_fss_sums(const double *S, int64_t P, int a0, int na, int b0, int nb, double *out, void *stream) {

@@ -119,21 +119,17 @@ extern "C" int b200_probability(const void *field, int dtype, int64_t plane_stri
                                 unsigned long long *scratch, double *out, void *stream) {
     B200_REQUIRE(T >= 0 && m >= 0 && n >= 0 && plane_stride >= 0 && scales != nullptr, "bad arguments");
     B200_REQUIRE((int64_t)m * n < ((int64_t)1 << 31), "probability: frames of 2^31 pixels or more are not supported");
-    if (T == 0 || (int64_t)m * n == 0) return 0;
-    B200_REQUIRE(field != nullptr && scratch != nullptr && out != nullptr, "bad arguments");
-    for (int t = 0; t < T; t++) {
-        B200_REQUIRE(scales[t] >= 0 && scales[t] <= B200_PROBABILITY_MAX_SCALE,
-                     "probability: kernel diameters must lie in 0 .. B200_PROBABILITY_MAX_SCALE");
-        B200_REQUIRE((int64_t)(m > n ? m : n) + scales[t] < ((int64_t)1 << 31), "probability: index range");
-        B200_REQUIRE(scales[t] == 0 || runs != nullptr, "bad arguments");
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    if (dtype == B200_F32)
-        return run<float>((const float *)field, plane_stride, T, m, n, threshold, nan_exceeds, scales, runs, scratch,
-                          out, s);
-    if (dtype == B200_F64)
-        return run<double>((const double *)field, plane_stride, T, m, n, threshold, nan_exceeds, scales, runs,
-                           scratch, out, s);
-    b200::set_error("probability: dtype must be B200_F32 or B200_F64");
-    return B200_EINVAL;
+    return b200::with_dtype("field", dtype, [&](auto tf) {
+        using F = typename decltype(tf)::type;
+        if (T == 0 || (int64_t)m * n == 0) return 0;
+        B200_REQUIRE(field != nullptr && scratch != nullptr && out != nullptr, "bad arguments");
+        for (int t = 0; t < T; t++) {
+            B200_REQUIRE(scales[t] >= 0 && scales[t] <= B200_PROBABILITY_MAX_SCALE,
+                         "probability: kernel diameters must lie in 0 .. B200_PROBABILITY_MAX_SCALE");
+            B200_REQUIRE((int64_t)(m > n ? m : n) + scales[t] < ((int64_t)1 << 31), "probability: index range");
+            B200_REQUIRE(scales[t] == 0 || runs != nullptr, "bad arguments");
+        }
+        return run<F>((const F *)field, plane_stride, T, m, n, threshold, nan_exceeds, scales, runs, scratch, out,
+                      (cudaStream_t)stream);
+    });
 }

@@ -247,7 +247,10 @@ __global__ void __launch_bounds__(THREADS)
         out[j] = j < n_nan ? (T)quiet_nan() : (T)picks[idx[m - 1 - (j - n_nan)]];
 }
 
-bool dtype_ok(int d) { return d == B200_F32 || d == B200_F64; }
+// the kernels here load either dtype at run time, so the entry points take only the visitor's check
+int check_dtypes(int a, int b) {
+    return b200::with_dtypes(a, b, [](auto, auto) { return 0; });
+}
 
 }  // namespace
 
@@ -263,9 +266,10 @@ extern "C" int b200_pm_match_stats(const void *x, int x_dtype, const unsigned ch
                                    void *stream) {
     const int64_t n = std::max(n_x, n_t);
     PmScratch s;
-    B200_REQUIRE(n_x >= 0 && n_t >= 0 && n < ((int64_t)1 << 31) && dtype_ok(x_dtype) && dtype_ok(t_dtype) && stats &&
-                     scratch && scratch_bytes >= carve(&s, nullptr, 0) && (n_x == 0 || x) && (n_t == 0 || t),
+    B200_REQUIRE(n_x >= 0 && n_t >= 0 && n < ((int64_t)1 << 31) && stats && scratch &&
+                     scratch_bytes >= carve(&s, nullptr, 0) && (n_x == 0 || x) && (n_t == 0 || t),
                  "bad arguments");
+    if (int rc = check_dtypes(x_dtype, t_dtype)) return rc;
     carve(&s, (char *)scratch, 0);
     cudaStream_t st = (cudaStream_t)stream;
     B200_CUDA(cudaMemsetAsync(s.head, 0, sizeof(Head), st));
@@ -287,9 +291,9 @@ extern "C" int b200_pm_match(const void *x, int x_dtype, const unsigned char *ig
                              void *stream) {
     PmScratch s;
     B200_REQUIRE(n >= 0 && n < ((int64_t)1 << 31) && n_xwet >= 0 && n_xwet <= n && n_twet >= 0 && n_twet <= n &&
-                     dtype_ok(x_dtype) && dtype_ok(t_dtype) &&
                      (!clip || (i0 >= 0 && i0 < n && i1 >= 0 && i1 < n)),
                  "bad arguments");
+    if (int rc = check_dtypes(x_dtype, t_dtype)) return rc;
     if (n == 0) return 0;
     B200_REQUIRE(x && t && stats && out && scratch && scratch_bytes >= carve(&s, nullptr, n), "bad arguments");
     carve(&s, (char *)scratch, n);
@@ -308,7 +312,8 @@ extern "C" int b200_pm_match(const void *x, int x_dtype, const unsigned char *ig
 
 extern "C" int b200_pm_resample_nan(const void *a, int a_dtype, const void *b, int b_dtype, int64_t n,
                                     int64_t *n_nan, void *stream) {
-    B200_REQUIRE(n >= 0 && n < ((int64_t)1 << 31) && dtype_ok(a_dtype) && dtype_ok(b_dtype) && n_nan, "bad arguments");
+    B200_REQUIRE(n >= 0 && n < ((int64_t)1 << 31) && n_nan, "bad arguments");
+    if (int rc = check_dtypes(a_dtype, b_dtype)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     B200_CUDA(cudaMemsetAsync(n_nan, 0, sizeof(int64_t), st));
     if (n == 0) return 0;
@@ -322,25 +327,26 @@ extern "C" int b200_pm_resample(const void *a, int a_dtype, const void *b, int b
                                 const unsigned char *draws, void *out, int out_dtype, void *scratch,
                                 int64_t scratch_bytes, void *stream) {
     PmScratch s;
-    B200_REQUIRE(n >= 0 && n < ((int64_t)1 << 31) && n_nan >= 0 && n_nan <= n && dtype_ok(a_dtype) &&
-                     dtype_ok(b_dtype) && dtype_ok(out_dtype),
-                 "bad arguments");
-    if (n == 0) return 0;
-    B200_REQUIRE(a && b && draws && out && scratch && scratch_bytes >= carve(&s, nullptr, n), "bad arguments");
-    carve(&s, (char *)scratch, n);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int64_t m = n - n_nan;
-    if (m) {
-        if (int rc = compact_sort(NotNan{a, a_dtype, b, b_dtype}, s.a, n, m, st)) return rc;
-        if (int rc = compact_sort(NotNan{b, b_dtype, a, a_dtype}, s.b, n, m, st)) return rc;
-        pick<<<grid_for(m), THREADS, 0, st>>>(a, a_dtype, b, b_dtype, s.a, s.b, m, n_nan, draws, s.picks);
+    B200_REQUIRE(n >= 0 && n < ((int64_t)1 << 31) && n_nan >= 0 && n_nan <= n, "bad arguments");
+    if (int rc = check_dtypes(a_dtype, b_dtype)) return rc;
+    return b200::with_dtype("output", out_dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        if (n == 0) return 0;
+        B200_REQUIRE(a && b && draws && out && scratch && scratch_bytes >= carve(&s, nullptr, n), "bad arguments");
+        carve(&s, (char *)scratch, n);
+        cudaStream_t st = (cudaStream_t)stream;
+        const int64_t m = n - n_nan;
+        if (m) {
+            if (int rc = compact_sort(NotNan{a, a_dtype, b, b_dtype}, s.a, n, m, st)) return rc;
+            if (int rc = compact_sort(NotNan{b, b_dtype, a, a_dtype}, s.b, n, m, st)) return rc;
+            pick<<<grid_for(m), THREADS, 0, st>>>(a, a_dtype, b, b_dtype, s.a, s.b, m, n_nan, draws, s.picks);
+            B200_LAUNCH_CHECK();
+            pick_keys<<<grid_for(m), THREADS, 0, st>>>(s.picks, m, s.a);
+            B200_LAUNCH_CHECK();
+            if (int rc = radix_sort(s.a, m, st)) return rc;
+        }
+        resample_out<T><<<grid_for(n), THREADS, 0, st>>>(s.picks, s.a, m, n_nan, (T *)out);
         B200_LAUNCH_CHECK();
-        pick_keys<<<grid_for(m), THREADS, 0, st>>>(s.picks, m, s.a);
-        B200_LAUNCH_CHECK();
-        if (int rc = radix_sort(s.a, m, st)) return rc;
-    }
-    if (out_dtype == B200_F32) resample_out<float><<<grid_for(n), THREADS, 0, st>>>(s.picks, s.a, m, n_nan, (float *)out);
-    else resample_out<double><<<grid_for(n), THREADS, 0, st>>>(s.picks, s.a, m, n_nan, (double *)out);
-    B200_LAUNCH_CHECK();
-    return 0;
+        return 0;
+    });
 }

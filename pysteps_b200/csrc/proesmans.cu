@@ -158,19 +158,13 @@ int consistency(const double *V, int h, int w, double *gamma, double *row_sum, l
 extern "C" int b200_proesmans_scale(const void *frames, int dtype, int64_t count, double im_min, double im_max,
                                     int do_scale, double *out, void *stream) {
     B200_REQUIRE(frames != nullptr && out != nullptr && count >= 1, "bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-    if (dtype == B200_F32)
-        scale_kernel<float><<<grid_for((size_t)count), 256, 0, s>>>((const float *)frames, out, (size_t)count, im_min,
-                                                                    im_max, do_scale);
-    else if (dtype == B200_F64)
-        scale_kernel<double><<<grid_for((size_t)count), 256, 0, s>>>((const double *)frames, out, (size_t)count, im_min,
-                                                                     im_max, do_scale);
-    else {
-        b200::set_error("unknown frame dtype %d", dtype);
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
-    return 0;
+    return b200::with_dtype("frame", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        scale_kernel<F><<<grid_for((size_t)count), 256, 0, (cudaStream_t)stream>>>((const F *)frames, out, (size_t)count,
+                                                                                    im_min, im_max, do_scale);
+        B200_LAUNCH_CHECK();
+        return 0;
+    });
 }
 
 extern "C" int b200_gaussian_filter(const double *in, int h, int w, const double *weights, int radius, double *out,

@@ -531,29 +531,6 @@ int velocity_pairs(const void *velocity, int layout, size_t N, b200::Scratch &bu
     return 0;
 }
 
-template <typename T> struct Type { using type = T; };
-
-// f(Type<float>{}) or f(Type<double>{}) for a dtype code (the entry points with one dtype take it for a velocity)
-template <typename Fn>
-int with_dtype(int dtype, Fn &&f) {
-    if (dtype == B200_F32) return f(Type<float>{});
-    if (dtype == B200_F64) return f(Type<double>{});
-    b200::set_error("unknown velocity dtype %d", dtype);
-    return B200_EINVAL;
-}
-
-// f(Type<FV>{}, Type<FP>{}) for the dtype codes of a velocity and a precipitation field
-template <typename Fn>
-int with_dtypes(int velocity_dtype, int precip_dtype, Fn &&f) {
-    const auto known = [](int d) { return d == B200_F32 || d == B200_F64; };
-    if (!known(velocity_dtype) || !known(precip_dtype)) {
-        b200::set_error("unknown field dtypes %d / %d", velocity_dtype, precip_dtype);
-        return B200_EINVAL;
-    }
-    return with_dtype(velocity_dtype,
-                      [&](auto fv) { return with_dtype(precip_dtype, [&](auto fp) { return f(fv, fp); }); });
-}
-
 // The argument rules the row-band entry points share, in the order they are checked.  `args_ok` and
 // `args_msg` are the entry point's own rule for its pointer arguments.
 int check_band(int m, int n, int row0, int rows, int layout, bool args_ok, const char *args_msg,
@@ -644,7 +621,7 @@ extern "C" int b200_sl_trajectories(const void *velocity, const double *xy_coord
                             "velocity / disp_steps is NULL", tdiff, T, n_iter, B200_MODE_CONSTANT))
         return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    return with_dtype(velocity_dtype, [&](auto fv) {
+    return b200::with_dtype("velocity", velocity_dtype, [&](auto fv) {
         using FV = typename decltype(fv)::type;
         b200::Scratch vi;
         const double2 *Vi;
@@ -667,7 +644,7 @@ extern "C" int b200_sl_extrapolate_rows(const void *precip, const void *velocity
     B200_REQUIRE((precip == nullptr) == (out == nullptr), "precip and out must both be given or both NULL");
     B200_REQUIRE(precip != nullptr || disp_out != nullptr, "nothing to compute");
     cudaStream_t s = (cudaStream_t)stream;
-    return with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
+    return b200::with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
         using FV = typename decltype(fv)::type;
         using F = typename decltype(fp)::type;
         const size_t N = (size_t)m * n;  // full frame (inputs)
@@ -706,7 +683,7 @@ extern "C" int b200_sl_extrapolate_rows_f32(const void *precip, const void *velo
         return B200_ENOTSUP;
     }
     cudaStream_t s = (cudaStream_t)stream;
-    return with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
+    return b200::with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
         using FV = typename decltype(fv)::type;
         using F = typename decltype(fp)::type;
         constexpr bool VF32 = sizeof(FV) == 4;
@@ -762,12 +739,15 @@ extern "C" int b200_sl_extrapolate_host(const void *precip, const void *velocity
                                         int n_iter, double outval, int mode, int velocity_dtype,
                                         int precip_dtype, int m, int n, void *out,
                                         double *disp_out) {
-    B200_REQUIRE(velocity_dtype == B200_F32 || velocity_dtype == B200_F64, "unknown velocity dtype");
-    B200_REQUIRE(precip_dtype == B200_F32 || precip_dtype == B200_F64, "unknown precip dtype");
+    size_t fs = 0, vs = 0;
+    if (int rc = b200::with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
+            vs = sizeof(typename decltype(fv)::type);
+            fs = sizeof(typename decltype(fp)::type);
+            return 0;
+        }))
+        return rc;
     B200_REQUIRE(velocity != nullptr && m >= 1 && n >= 1 && T >= 1, "bad arguments");
     const size_t N = (size_t)m * n;
-    const size_t fs = precip_dtype == B200_F32 ? 4 : 8;
-    const size_t vs = velocity_dtype == B200_F32 ? 4 : 8;
     cudaStream_t s = nullptr;
     b200::Scratch dP, dV, dXY, dDP, dOut, dDO;
     B200_CUDA(dV.alloc(2 * N * vs, s));
@@ -805,7 +785,7 @@ extern "C" int b200_sl_interleave_velocity(const void *velocity, int velocity_dt
     B200_REQUIRE(velocity != nullptr && out != nullptr && m >= 1 && n >= 1, "bad arguments");
     const size_t N = (size_t)m * n;
     cudaStream_t s = (cudaStream_t)stream;
-    return with_dtype(velocity_dtype, [&](auto fv) {
+    return b200::with_dtype("velocity", velocity_dtype, [&](auto fv) {
         using F = typename decltype(fv)::type;
         using F2 = std::conditional_t<sizeof(F) == 4, float2, double2>;
         relayout_kernel<F, F2, false><<<stream_blocks(N, 16), 256, 0, s>>>((const F *)velocity, (F2 *)out, N);
@@ -931,7 +911,7 @@ extern "C" int b200_sl_step_batched(const void *velocity, int velocity_dtype, in
     B200_REQUIRE(m >= 1 && n >= 1 && (int64_t)m * n < ((int64_t)1 << 30) && members >= 1, "bad sizes");
     B200_REQUIRE(mode == B200_MODE_CONSTANT || mode == B200_MODE_NEAREST, "unsupported mode");
     cudaStream_t s = (cudaStream_t)stream;
-    return with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
+    return b200::with_dtypes(velocity_dtype, precip_dtype, [&](auto fv, auto fp) {
         using FV = typename decltype(fv)::type;
         using F = typename decltype(fp)::type;
         const size_t N = (size_t)m * n;
@@ -982,7 +962,7 @@ extern "C" int b200_bps_perturb_velocity(const void *velocity, int velocity_dtyp
     B200_REQUIRE(velocity != nullptr && out != nullptr && m >= 1 && n >= 1, "bad arguments");
     const size_t N = (size_t)m * n;
     cudaStream_t s = (cudaStream_t)stream;
-    return with_dtype(velocity_dtype, [&](auto fv) {
+    return b200::with_dtype("velocity", velocity_dtype, [&](auto fv) {
         return bps_launch<typename decltype(fv)::type>(velocity, N, a_par, a_perp, vsf, what, out, n_nonfinite, s);
     });
 }

@@ -87,17 +87,14 @@ extern "C" int b200_spline_prepare(const void *precip, int precip_dtype, int m, 
     const size_t total = (size_t)M * N;
     const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)b200::num_sms() * 16);
     const int want_masks = order > 1;
-    if (precip_dtype == B200_F32)
-        spline_prepare_kernel<float><<<blocks, 256, 0, s>>>((const float *)precip, m, n, pad, stats, zero_fill,
-                                                             want_masks, coeffs, mask_min, mask_finite);
-    else if (precip_dtype == B200_F64)
-        spline_prepare_kernel<double><<<blocks, 256, 0, s>>>((const double *)precip, m, n, pad, stats, zero_fill,
-                                                              want_masks, coeffs, mask_min, mask_finite);
-    else {
-        b200::set_error("unknown precip dtype %d", precip_dtype);
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
+    if (int rc = b200::with_dtype("precip", precip_dtype, [&](auto t) {
+            using F = typename decltype(t)::type;
+            spline_prepare_kernel<F><<<blocks, 256, 0, s>>>((const F *)precip, m, n, pad, stats, zero_fill, want_masks,
+                                                             coeffs, mask_min, mask_finite);
+            B200_LAUNCH_CHECK();
+            return 0;
+        }))
+        return rc;
     if (order <= 1) return 0;
     spl::FilterParams f0;
     memset(&f0, 0, sizeof(f0));
@@ -150,15 +147,9 @@ extern "C" int b200_spline_sample(const double *coeffs, int m, int n, int order,
     p.row0 = row_begin; p.rows = row_count;
     p.cval = outval;
     dim3 block(32, 4), grid(b200::ceil_div(n, 32), b200::ceil_div(row_count, 4), T);
-    cudaStream_t s = (cudaStream_t)stream;
-    if (out_dtype == B200_F32)
-        spline_sample_kernel<float><<<grid, block, 0, s>>>(p);
-    else if (out_dtype == B200_F64)
-        spline_sample_kernel<double><<<grid, block, 0, s>>>(p);
-    else {
-        b200::set_error("unknown output dtype %d", out_dtype);
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
-    return 0;
+    return b200::with_dtype("output", out_dtype, [&](auto t) {
+        spline_sample_kernel<typename decltype(t)::type><<<grid, block, 0, (cudaStream_t)stream>>>(p);
+        B200_LAUNCH_CHECK();
+        return 0;
+    });
 }

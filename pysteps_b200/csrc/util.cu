@@ -1,5 +1,5 @@
 // util.cu -- field statistics (validation of semilagrangian.py:112-123,171-172)
-// and dtype conversion.  Pure streaming, HBM-bound: 16-byte loads, grid sized
+// and a float64 fill.  Pure streaming, HBM-bound: 16-byte loads, grid sized
 // to a multiple of the SM count, deterministic two-stage reduction.
 #include <math_constants.h>
 
@@ -100,14 +100,6 @@ __global__ void __launch_bounds__(256) stats_final_kernel(const Stats *__restric
     }
 }
 
-template <typename S, typename D>
-__global__ void __launch_bounds__(256) convert_kernel(const S *__restrict__ src, D *__restrict__ dst,
-                                                      int64_t count) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride)
-        dst[i] = (D)src[i];
-}
-
 __global__ void __launch_bounds__(256) fill_kernel(double *__restrict__ dst, int64_t count, double v) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride) dst[i] = v;
@@ -127,43 +119,17 @@ extern "C" int b200_fill_f64(double *dst, int64_t count, double value, void *str
 extern "C" int b200_field_stats(const void *a, int field_dtype, int64_t count, double *stats,
                                 void *stream) {
     B200_REQUIRE(a != nullptr && stats != nullptr && count >= 0, "bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-    const int blocks = (int)std::max<int64_t>(
-        1, std::min<int64_t>(b200::ceil_div64(count, 256 * 4), (int64_t)b200::num_sms() * 8));
-    b200::Scratch part;
-    B200_CUDA(part.alloc(sizeof(Stats) * blocks, s));
-    if (field_dtype == B200_F32)
-        stats_partial_kernel<float><<<blocks, 256, 0, s>>>((const float *)a, count, (Stats *)part.p);
-    else if (field_dtype == B200_F64)
-        stats_partial_kernel<double><<<blocks, 256, 0, s>>>((const double *)a, count, (Stats *)part.p);
-    else {
-        b200::set_error("unknown field dtype %d", field_dtype);
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
-    stats_final_kernel<<<1, 256, 0, s>>>((const Stats *)part.p, blocks, stats);
-    B200_LAUNCH_CHECK();
-    return 0;
-}
-
-extern "C" int b200_convert(const void *src, int src_dtype, void *dst, int dst_dtype, int64_t count,
-                            void *stream) {
-    B200_REQUIRE(src != nullptr && dst != nullptr && count >= 0, "bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-    const int blocks = (int)std::max<int64_t>(
-        1, std::min<int64_t>(b200::ceil_div64(count, 256), (int64_t)b200::num_sms() * 16));
-    if (src_dtype == B200_F64 && dst_dtype == B200_F32)
-        convert_kernel<double, float><<<blocks, 256, 0, s>>>((const double *)src, (float *)dst, count);
-    else if (src_dtype == B200_F32 && dst_dtype == B200_F64)
-        convert_kernel<float, double><<<blocks, 256, 0, s>>>((const float *)src, (double *)dst, count);
-    else if (src_dtype == dst_dtype && (src_dtype == B200_F32 || src_dtype == B200_F64)) {
-        B200_CUDA(cudaMemcpyAsync(dst, src, (size_t)count * (src_dtype == B200_F32 ? 4 : 8),
-                                  cudaMemcpyDeviceToDevice, s));
+    return b200::with_dtype("field", field_dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        cudaStream_t s = (cudaStream_t)stream;
+        const int blocks = (int)std::max<int64_t>(
+            1, std::min<int64_t>(b200::ceil_div64(count, 256 * 4), (int64_t)b200::num_sms() * 8));
+        b200::Scratch part;
+        B200_CUDA(part.alloc(sizeof(Stats) * blocks, s));
+        stats_partial_kernel<F><<<blocks, 256, 0, s>>>((const F *)a, count, (Stats *)part.p);
+        B200_LAUNCH_CHECK();
+        stats_final_kernel<<<1, 256, 0, s>>>((const Stats *)part.p, blocks, stats);
+        B200_LAUNCH_CHECK();
         return 0;
-    } else {
-        b200::set_error("unsupported conversion %d -> %d", src_dtype, dst_dtype);
-        return B200_EINVAL;
-    }
-    B200_LAUNCH_CHECK();
-    return 0;
+    });
 }

@@ -480,43 +480,34 @@ int roc_run(const F *P, const O *obs, int64_t N, const double *thr, int n_thr, d
     return 0;
 }
 
-bool float_code(int c) { return c == B200_F32 || c == B200_F64; }
-
-// RUN(F, O) for the four dtype pairs of (a, b)
-#define B200_DISPATCH2(a, b, RUN)                                          \
-    do {                                                                   \
-        if ((a) == B200_F32 && (b) == B200_F32) return RUN(float, float);  \
-        if ((a) == B200_F32) return RUN(float, double);                    \
-        if ((b) == B200_F32) return RUN(double, float);                    \
-        return RUN(double, double);                                        \
-    } while (0)
-
 }  // namespace
 
 extern "C" int b200_pairwise_sum(const void *x, int dtype, const int64_t *seg_off, const int64_t *seg_len, int nseg,
                                  void *out, void *stream) {
-    B200_REQUIRE(nseg >= 0 && float_code(dtype), "pairwise_sum: bad arguments");
-    if (nseg == 0) return 0;
-    B200_REQUIRE(seg_off != nullptr && seg_len != nullptr && out != nullptr, "pairwise_sum: bad arguments");
-    cudaStream_t s = (cudaStream_t)stream;
-    if (dtype == B200_F32) return pairwise_run<float>((const float *)x, seg_off, seg_len, nseg, (float *)out, s);
-    return pairwise_run<double>((const double *)x, seg_off, seg_len, nseg, (double *)out, s);
+    B200_REQUIRE(nseg >= 0, "pairwise_sum: bad arguments");
+    return b200::with_dtype("field", dtype, [&](auto t) {
+        using F = typename decltype(t)::type;
+        if (nseg == 0) return 0;
+        B200_REQUIRE(seg_off != nullptr && seg_len != nullptr && out != nullptr, "pairwise_sum: bad arguments");
+        return pairwise_run<F>((const F *)x, seg_off, seg_len, nseg, (F *)out, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200_verif_crps(const void *Xf, int f_dtype, const void *Xo, int o_dtype, int k, int64_t N,
                                double *res, int64_t *n, void *stream) {
     B200_REQUIRE(k >= 1 && k <= B200_VERIF_MAX_MEMBERS && N >= 0 && N < ((int64_t)1 << 31) && n != nullptr,
                  "verif_crps: bad arguments");
-    B200_REQUIRE(float_code(f_dtype) && float_code(o_dtype), "verif_crps: dtypes must be B200_F32 or B200_F64");
     cudaStream_t s = (cudaStream_t)stream;
-    if (N == 0) {
-        B200_CUDA(cudaMemsetAsync(n, 0, sizeof(int64_t), s));
-        return 0;
-    }
-    B200_REQUIRE(Xf != nullptr && Xo != nullptr && res != nullptr, "verif_crps: bad arguments");
-#define B200_RUN(F, O) crps_run<F, O>((const F *)Xf, (const O *)Xo, k, N, res, n, s)
-    B200_DISPATCH2(f_dtype, o_dtype, B200_RUN);
-#undef B200_RUN
+    return b200::with_dtypes(f_dtype, o_dtype, [&](auto tf, auto to) {
+        using F = typename decltype(tf)::type;
+        using O = typename decltype(to)::type;
+        if (N == 0) {
+            B200_CUDA(cudaMemsetAsync(n, 0, sizeof(int64_t), s));
+            return 0;
+        }
+        B200_REQUIRE(Xf != nullptr && Xo != nullptr && res != nullptr, "verif_crps: bad arguments");
+        return crps_run<F, O>((const F *)Xf, (const O *)Xo, k, N, res, n, s);
+    });
 }
 
 extern "C" int b200_verif_rankhist(const void *Xf, int f_dtype, const void *Xo, int o_dtype, int k, int64_t N,
@@ -525,18 +516,19 @@ extern "C" int b200_verif_rankhist(const void *Xf, int f_dtype, const void *Xo, 
     B200_REQUIRE(k >= 1 && k <= B200_VERIF_MAX_MEMBERS && N >= 0 && N < ((int64_t)1 << 31) && hist != nullptr &&
                      n_ties != nullptr,
                  "verif_rankhist: bad arguments");
-    B200_REQUIRE(float_code(f_dtype) && float_code(o_dtype), "verif_rankhist: dtypes must be B200_F32 or B200_F64");
     cudaStream_t s = (cudaStream_t)stream;
-    if (N == 0) {
-        B200_CUDA(cudaMemsetAsync(hist, 0, sizeof(int64_t) * (k + 1), s));
-        B200_CUDA(cudaMemsetAsync(n_ties, 0, sizeof(int64_t), s));
-        return 0;
-    }
-    B200_REQUIRE(Xf != nullptr && Xo != nullptr && ties != nullptr, "verif_rankhist: bad arguments");
-#define B200_RUN(F, O) \
-    rankhist_run<F, O>((const F *)Xf, (const O *)Xo, k, N, use_min, thr_f, sub_f, thr_o, sub_o, hist, ties, n_ties, s)
-    B200_DISPATCH2(f_dtype, o_dtype, B200_RUN);
-#undef B200_RUN
+    return b200::with_dtypes(f_dtype, o_dtype, [&](auto tf, auto to) {
+        using F = typename decltype(tf)::type;
+        using O = typename decltype(to)::type;
+        if (N == 0) {
+            B200_CUDA(cudaMemsetAsync(hist, 0, sizeof(int64_t) * (k + 1), s));
+            B200_CUDA(cudaMemsetAsync(n_ties, 0, sizeof(int64_t), s));
+            return 0;
+        }
+        B200_REQUIRE(Xf != nullptr && Xo != nullptr && ties != nullptr, "verif_rankhist: bad arguments");
+        return rankhist_run<F, O>((const F *)Xf, (const O *)Xo, k, N, use_min, thr_f, sub_f, thr_o, sub_o, hist, ties,
+                                  n_ties, s);
+    });
 }
 
 extern "C" int b200_verif_rankhist_ties(const void *ties, int64_t n_ties, const double *u, int k, int64_t *hist,
@@ -557,18 +549,18 @@ extern "C" int b200_verif_reldiag(const void *P, int p_dtype, const void *Xo, in
     B200_REQUIRE(N >= 0 && N < ((int64_t)1 << 31) && n_edges >= 1 && n_edges <= B200_VERIF_MAX_BINS + 1 &&
                      edges != nullptr && seg != nullptr && above != nullptr,
                  "verif_reldiag: bad arguments");
-    B200_REQUIRE(float_code(p_dtype) && float_code(o_dtype), "verif_reldiag: dtypes must be B200_F32 or B200_F64");
     cudaStream_t s = (cudaStream_t)stream;
-    if (N == 0) {
-        B200_CUDA(cudaMemsetAsync(seg, 0, sizeof(int64_t) * n_edges, s));
-        B200_CUDA(cudaMemsetAsync(above, 0, sizeof(int64_t) * std::max(n_edges - 1, 1), s));
-        return 0;
-    }
-    B200_REQUIRE(P != nullptr && Xo != nullptr && sorted != nullptr, "verif_reldiag: bad arguments");
-#define B200_RUN(F, O) \
-    reldiag_run<F, O>((const F *)P, (const O *)Xo, N, edges, n_edges, thr_o, (F *)sorted, seg, above, s)
-    B200_DISPATCH2(p_dtype, o_dtype, B200_RUN);
-#undef B200_RUN
+    return b200::with_dtypes(p_dtype, o_dtype, [&](auto tp, auto to) {
+        using F = typename decltype(tp)::type;
+        using O = typename decltype(to)::type;
+        if (N == 0) {
+            B200_CUDA(cudaMemsetAsync(seg, 0, sizeof(int64_t) * n_edges, s));
+            B200_CUDA(cudaMemsetAsync(above, 0, sizeof(int64_t) * std::max(n_edges - 1, 1), s));
+            return 0;
+        }
+        B200_REQUIRE(P != nullptr && Xo != nullptr && sorted != nullptr, "verif_reldiag: bad arguments");
+        return reldiag_run<F, O>((const F *)P, (const O *)Xo, N, edges, n_edges, thr_o, (F *)sorted, seg, above, s);
+    });
 }
 
 extern "C" int b200_verif_roc(const void *P, int p_dtype, const void *Xo, int o_dtype, int64_t N, const double *thr,
@@ -576,14 +568,15 @@ extern "C" int b200_verif_roc(const void *P, int p_dtype, const void *Xo, int o_
     B200_REQUIRE(N >= 0 && N < ((int64_t)1 << 31) && n_thr >= 0 && n_thr <= B200_VERIF_MAX_BINS &&
                      counts != nullptr && (n_thr == 0 || thr != nullptr),
                  "verif_roc: bad arguments");
-    B200_REQUIRE(float_code(p_dtype) && float_code(o_dtype), "verif_roc: dtypes must be B200_F32 or B200_F64");
     cudaStream_t s = (cudaStream_t)stream;
-    if (N == 0) {
-        B200_CUDA(cudaMemsetAsync(counts, 0, sizeof(int64_t) * 2 * (n_thr + 1), s));
-        return 0;
-    }
-    B200_REQUIRE(P != nullptr && Xo != nullptr, "verif_roc: bad arguments");
-#define B200_RUN(F, O) roc_run<F, O>((const F *)P, (const O *)Xo, N, thr, n_thr, thr_o, counts, s)
-    B200_DISPATCH2(p_dtype, o_dtype, B200_RUN);
-#undef B200_RUN
+    return b200::with_dtypes(p_dtype, o_dtype, [&](auto tp, auto to) {
+        using F = typename decltype(tp)::type;
+        using O = typename decltype(to)::type;
+        if (N == 0) {
+            B200_CUDA(cudaMemsetAsync(counts, 0, sizeof(int64_t) * 2 * (n_thr + 1), s));
+            return 0;
+        }
+        B200_REQUIRE(P != nullptr && Xo != nullptr, "verif_roc: bad arguments");
+        return roc_run<F, O>((const F *)P, (const O *)Xo, N, thr, n_thr, thr_o, counts, s);
+    });
 }
